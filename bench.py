@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py - throughput of the decode -> sample -> preprocess -> embed/classify hot path on B200.
+"""bench.py - throughput of the decode -> sample -> preprocess -> embed/classify hot path on H100.
 
     python bench.py --gpus 1 --steps K --warmup W                 # this repo's CUDA path
     python bench.py --impl reference --gpus 1 --steps K --warmup W # the reference's CPU path (oracle) on host cores
@@ -19,11 +19,15 @@ Printed JSON line (rank 0):
           sampled one (the reference's decode semantics) + fused preprocess + tower + pinned D2H of scores/embeddings, the decode /
           tower overlap happening inside the stage; wall clock between device synchronisations, max over ranks.
   e2e_keyframe_seek  the same call with seek_keyframes=True (opt-in: identical frames, only GOPs with sampled frames are decoded).
-  roofline      the dominant kernel (tcgen05 GEMM): algorithmic FLOPs per launch / CUDA-event time per launch vs the
-                measured sustained bf16 peak (MEASURED_PEAKS.json); roofline_other has preprocess / LayerNorm (HBM).
+  roofline      the dominant kernel (wgmma GEMM): algorithmic FLOPs per launch / CUDA-event time per launch vs the
+                peak in MEASURED_PEAKS.json (else the H100 SXM data-sheet figure); roofline_other has preprocess / LayerNorm (HBM).
   cpu_baseline  the oracle's CPU restatement of the reference path timed on the host cores (N=1, rank 0), bounded sample.
   gpu_library_baseline  the reference's GPU *library* path restated without Ray (torch-CUDA torchvision transforms + HF CLIPModel
                 fp32, one call per clip, clip.py:36-74 / aesthetic_filter_stages.py:181-183), N=1 rank 0, bounded sample.
+
+`--dump-outputs DIR` writes what the last timed step of the `value` path returned (embedding.npy, score.npy; float32) so that two
+builds can be compared output for output: the clips, the sampling plan and the weights are seeded, the same arguments give the
+same inputs.
 """
 
 from __future__ import annotations
@@ -33,6 +37,7 @@ import json
 import os
 import subprocess
 import sys
+import tempfile
 import threading
 import time
 from pathlib import Path
@@ -45,7 +50,7 @@ import numpy as np  # noqa: E402
 
 FRAME_W, FRAME_H, FPS, SECONDS = 1920, 1080, 30, 10.0
 SAMPLE_FPS = 1.0
-FALLBACK_PEAKS = {"hbm_gbs": 6650.0, "bf16_tflops": 1590.0, "bf16_tflops_sustained": 1400.0}
+FALLBACK_PEAKS = {"hbm_gbs": 3350.0, "bf16_tflops": 989.0}  # NVIDIA data sheet, H100 SXM at 700 W (dense); not measured
 
 
 def peaks() -> tuple[dict, str]:
@@ -56,7 +61,7 @@ def peaks() -> tuple[dict, str]:
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons during the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons during the timed region."""
 
     Q = "index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap"
 
@@ -112,10 +117,10 @@ def _gen_clip(args) -> str:
 
 def make_clips(n_distinct: int, rank: int, workers: int | None = None, size: tuple[int, int] = (FRAME_W, FRAME_H), bitrate: float = BITRATE) -> list[bytes]:
     """`n_distinct` residual-coded clips (seed = 1000 * rank + i), generated by a fork pool BEFORE CUDA is initialised and
-    cached under /tmp (both arms of one box reuse them)."""
+    cached under the temporary directory (both arms of one machine reuse them)."""
     import multiprocessing as mp
 
-    root = os.path.join(os.environ.get("CB_CLIP_CACHE", "/tmp"), f"cb_clips_{size[0]}x{size[1]}_{FPS}_{int(SECONDS)}s_{int(bitrate)}")
+    root = os.path.join(os.environ.get("CB_CLIP_CACHE", tempfile.gettempdir()), f"cb_clips_{size[0]}x{size[1]}_{FPS}_{int(SECONDS)}s_{int(bitrate)}")
     os.makedirs(root, exist_ok=True)
     jobs = [(1000 * rank + i, os.path.join(root, f"clip_{1000 * rank + i}.mp4"), size[0], size[1], bitrate) for i in range(n_distinct)]
     todo = [j for j in jobs if not os.path.exists(j[1])]
@@ -221,7 +226,7 @@ def run_b200(args) -> None:
     from cosmos_curate_b200.data_model import Clip, SplitPipeTask, Video
     from cosmos_curate_b200.models import weights as W
     from cosmos_curate_b200.models.clip_aesthetics import CLIPAestheticScorer
-    from cosmos_curate_b200.runtime import alloc_nv12_pool, decode_discard, get_context, mp4_index
+    from cosmos_curate_b200.runtime import alloc_nv12_pool, decode_discard, get_context, mp4_index, nvdec_available
     from cosmos_curate_b200.stages import NvdecClipAestheticStage
 
     cfg = W.CLIP_VIT_L14
@@ -247,6 +252,12 @@ def run_b200(args) -> None:
 
     stage = make_stage(seek=False)
     ctx = get_context()
+    hw_decode = nvdec_available(ctx)
+    if not hw_decode:
+        # NVDEC is not usable from this process (runtime.nvdec_available has warned): clips are decoded on the host.  That feeds the
+        # resident-input measurement the same surfaces, but the end-to-end and secondary rows exist to measure the hardware decoder.
+        print("bench: NVDEC not usable, e2e and secondary rows are NOT measured", file=sys.stderr)
+        args.no_e2e = args.no_secondary = True
     tower = model.tower
 
     def make_tasks(call: int) -> list:
@@ -302,6 +313,10 @@ def run_b200(args) -> None:
     dev_s = max_over_ranks(ev0.elapsed_time(ev1) / 1e3)
     launches = ctx.launch_count() - l0
     value = world * cps * args.steps / dev_s
+    if args.dump_outputs and rank == 0:  # what a caller of embed_pool received in the last timed step (its second value, the un-normalised features, is only produced on request)
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        np.save(os.path.join(args.dump_outputs, "embedding.npy"), emb.float().cpu().numpy().astype(np.float32))
+        np.save(os.path.join(args.dump_outputs, "score.npy"), score.float().cpu().numpy().astype(np.float32))
     del pool0
 
     # ---- end-to-end measurement (e2e): the product stage on host tasks
@@ -426,11 +441,10 @@ def run_b200(args) -> None:
         return
 
     pk, pk_src = peaks()
-    traffic = ncu_traffic()
     gemm_flops = cfg.gemm_flops_per_image() * frames_per_step * args.steps
     gemm_ms, gemm_n = prof["gemm"]["ms"], max(1, prof["gemm"]["launches"])
     ach_tf = gemm_flops / (gemm_ms / 1e3) / 1e12 if gemm_ms > 0 else 0.0
-    peak_tf = pk.get("bf16_tflops_sustained", pk["bf16_tflops"])
+    peak_tf = pk["bf16_tflops"]
     pre_bytes = (1.5 * min(FRAME_W, FRAME_H) ** 2 + 3 * 224 * 224 * 2) * frames_per_step * args.steps
     ln_bytes = 6.0 * cfg.tokens * cfg.hidden * frames_per_step * (2 * cfg.layers) * args.steps  # fp32 in + fp16 out per LayerNorm
     other = {}
@@ -438,7 +452,6 @@ def run_b200(args) -> None:
         ms = prof[key]["ms"]
         gbs = nbytes / (ms / 1e3) / 1e9 if ms > 0 else 0.0
         other[name] = {"bound": "hbm", "achieved": gbs, "peak": pk["hbm_gbs"], "unit": "GB/s", "frac": gbs / pk["hbm_gbs"],
-                       "traffic": traffic.get({"preprocess": "clip_preprocess", "layernorm": "layernorm_kernel"}[name]),
                        "ms_per_step": ms / args.steps, "launches_per_step": prof[key]["launches"] / args.steps}  # fmt: skip
     other["attention"] = {"ms_per_step": prof["attention"]["ms"] / args.steps, "launches_per_step": prof["attention"]["launches"] / args.steps}
     step_ms = 1e3 * dev_s / args.steps
@@ -446,16 +459,15 @@ def run_b200(args) -> None:
         "metric": "clips_per_sec", "value": value, "unit": "clips/s", "n_gpus": world, "steps": args.steps, "warmup": max(args.warmup, 3), "ms_per_step": step_ms,
         "higher_is_better": True, "scaling": "weak", "vs_baseline": None, "dtype": "f16", "data": "synthetic",
         "frames_per_sec": world * frames_per_step * args.steps / dev_s,
-        "config": {"workload": WORKLOAD, "implementation": "one process per B200: NVDEC + fused preprocess kernel + tcgen05 tower behind NvdecClipAestheticStage",
+        "config": {"workload": WORKLOAD, "implementation": "one process per H100: NVDEC + fused preprocess kernel + wgmma tower behind NvdecClipAestheticStage",
                    "clips_per_step": cps, "frames_per_clip": fpc, "frames_per_step": frames_per_step, "sample_fps": SAMPLE_FPS, "distinct_clips": args.distinct_clips,
                    "clip_bitrate_bps": float(np.mean([8 * len(c) / SECONDS for c in clips])),
                    "clip_stream": "tools/synth_h264.make_coded_clip: Intra16x16 IDR (DC + sparse AC, chroma DC) + P (P_Skip runs, quarter-pel 16x16 motion, sparse 4x4 residuals), CAVLC, deblocking on, GOP 30",
                    "network": "clip-vit-large-patch14, seeded random weights, fp16 operands / fp32 accumulate+residual", "sharding": f"{world} rank(s), clips sharded per rank, no data-path collective",
-                   "l2": "inputs (NV12 pool 0.88 GB + activations > 1 GB) exceed the 126 MB L2", "value_inputs": "decoded NV12 surfaces resident in HBM"},
+                   "l2": "inputs (NV12 pool 0.88 GB + activations > 1 GB) exceed the 50 MB L2", "value_inputs": "decoded NV12 surfaces resident in HBM"},
         "clocks": clocks, "gpu_launches": int(launches),
-        "roofline": {"bound": "tensor", "kernel": "gemm_tcgen05_2cta_kernel", "achieved": ach_tf, "peak": peak_tf, "unit": "TFLOP/s", "frac": ach_tf / peak_tf,
-                     "traffic": traffic.get("gemm_tcgen05_2cta"), "traffic_source": traffic.get("_source"),
-                     "peak_source": f"{pk_src} bf16_tflops_sustained (kernel timed inside a long step)", "launches_per_step": gemm_n / args.steps,
+        "roofline": {"bound": "tensor", "kernel": "gemm_wgmma_kernel", "achieved": ach_tf, "peak": peak_tf, "unit": "TFLOP/s", "frac": ach_tf / peak_tf,
+                     "peak_source": f"{pk_src} fp16/bf16 dense peak (kernel timed inside a long step)", "launches_per_step": gemm_n / args.steps,
                      "ms_per_step": gemm_ms / args.steps, "share_of_step": gemm_ms / args.steps / step_ms},
         "roofline_other": other,
         "e2e": e2e, "e2e_keyframe_seek": e2e_sparse, "decode_roofline": ceiling, "host": host_cpu_info(),
@@ -468,6 +480,8 @@ def run_b200(args) -> None:
             shot["fp32_peak_tflops"] = peak
             shot["frac_of_fp32_peak"] = shot["tflops_fp32"] / peak
         line["shot_detection"] = shot
+    if not hw_decode:
+        e2e_error = "not measured: NVDEC is not usable from this process (cuvidGetDecoderCaps reports no H.264 support); the clips of the value path were decoded on the host"
     if e2e_error:
         line["e2e_error"] = e2e_error
     if world == 1 and not args.no_secondary:
@@ -533,7 +547,7 @@ def secondary_configs(ctx, torch, clips_1080p: list[bytes], clips_4k, args, clip
         st.destroy()
         model.tower.close()
         out["c1"] = {"workload": "32 x (854x480 24 fps 5 s H.264 High/CABAC real content: the reference's test fixture cut to 5 s by stream copy) -> 1 fps -> CLIP ViT-B/32 (seeded) + aesthetic head "
-                                 "(BASELINE.json configs[0])", "b200_e2e_clips_per_sec": cps, "clips": n, "api": "NvdecClipAestheticStage.process_data, host mp4 bytes in",
+                                 "(BASELINE.json configs[0])", "e2e_clips_per_sec": cps, "clips": n, "api": "NvdecClipAestheticStage.process_data, host mp4 bytes in",
                      "cpu": cpu_c1(c1)}  # fmt: skip
 
     # ---- C4-shaped: 4K clips, 2 fps sampling, SoViT-400m/14 @384 embedding-only (HEVC streams cannot be produced here: H.264 at 4K instead)
@@ -573,7 +587,7 @@ def secondary_configs(ctx, torch, clips_1080p: list[bytes], clips_4k, args, clip
             "workload": "3840x2160 30 fps 10 s H.264 ~16 Mb/s synthetic clips (HEVC cannot be produced in this image; NVDEC accepts hvc1/hev1) -> 2 fps (21 frames/clip) -> "
                         "SigLIP SoViT-400m/14 @384 embedding, seeded weights (BASELINE.json configs[3] shape, one GPU)",
             "e2e_clips_per_sec": cps, "clips": n, "decoded_frames_per_call": decoded, "resident_frames_per_sec": 84 / ms * 1e3, "resident_ms_per_84_frames": ms,
-            "gemm": {"achieved_tflops": gemm_tf, "peak": pk.get("bf16_tflops_sustained", pk["bf16_tflops"]), "frac": gemm_tf / pk.get("bf16_tflops_sustained", pk["bf16_tflops"]),
+            "gemm": {"achieved_tflops": gemm_tf, "peak": pk["bf16_tflops"], "frac": gemm_tf / pk["bf16_tflops"],
                      "ms": prof["gemm"]["ms"] / reps},
             "attention_ms": prof["attention"]["ms"] / reps, "layernorm_ms": prof["layernorm"]["ms"] / reps,
             "preprocess": {"ms": prof["preprocess"]["ms"] / reps, "algorithmic_gbs": pre_b / (prof["preprocess"]["ms"] / 1e3) / 1e9},
@@ -763,26 +777,11 @@ def shot_detection_measure(ctx, torch, n_frames: int = 9000, reps: int = 3) -> d
 WORKLOAD = "1080p30 10 s H.264 clips -> 1 fps frame sampling -> preprocess -> CLIP-ViT-L/14 embed + aesthetic score (BASELINE.json configs[1])"
 
 
-def ncu_traffic() -> dict:
-    """DRAM bytes per launch from the committed `ncu --set full` capture (profiles/rNN_traffic.json, newest round); {} if none."""
-    import glob
-
-    files = sorted(glob.glob(os.path.join(os.path.dirname(os.path.abspath(__file__)), "profiles", "r*_traffic.json")))
-    if not files:
-        return {}
-    with open(files[-1]) as f:
-        d = json.load(f)
-    out = {k: v["traffic_bytes_per_launch"] for k, v in d["kernels"].items()}
-    out["_source"] = os.path.join("profiles", os.path.basename(files[-1]))
-    return out
-
-
 def cpu_layout(cores: int) -> tuple[int, int]:
     """(worker processes, torch threads each): the reference scales this path by replicating actors, not by threading one model."""
     if os.environ.get("CB_REF_PROCS") and os.environ.get("CB_REF_THREADS"):  # tuning override
         return int(os.environ["CB_REF_PROCS"]), int(os.environ["CB_REF_THREADS"])
-    # measured on the 128-thread (64-core) B200 host: 16 workers x 4 threads = 0.58 clips/s, 8 x 8 = 0.51, 8 x 16 = 0.27-0.32,
-    # 16 x 8 = 0.36, 4 x 32 = 0.19 -> one torch thread per PHYSICAL core, four per worker
+    # one torch thread per PHYSICAL core, four per worker
     if cores >= 32:
         return cores // 8, 4
     return max(1, cores // 4), min(4, cores) if cores >= 4 else 1
@@ -819,13 +818,16 @@ def main() -> None:
     ap.add_argument("--ceiling-seconds", type=float, default=5.0, help="duration of the decode-only ceiling measurement")
     ap.add_argument("--no-secondary", action="store_true", help="skip the C1 / C4-shaped / clip-cut secondary rows")
     ap.add_argument("--no-gpu-library", action="store_true", help="skip the reference GPU library-path baseline")
-    ap.add_argument("--decoders", type=int, default=20, help="concurrent NVDEC sessions per GPU (7 engines on B200)")
+    ap.add_argument("--decoders", type=int, default=20, help="concurrent NVDEC sessions per GPU (7 NVDEC engines on H100)")
     ap.add_argument("--e2e-steps", type=int, default=2, help="timed process_data calls of the e2e measurement")
     ap.add_argument("--ref-clips", type=int, default=2, help="clips per step of the reference arm (bounded sample)")
     ap.add_argument("--no-shots", action="store_true", help="skip the shot-detection secondary measurement")
     ap.add_argument("--no-e2e", action="store_true")
     ap.add_argument("--no-cpu-baseline", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None, help="write the arrays the last timed step returned as DIR/<name>.npy (float32)")
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be at least 1")
     if args.impl == "reference":
         run_reference(args)
     else:

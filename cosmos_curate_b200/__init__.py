@@ -1,7 +1,7 @@
-"""cosmos_curate_b200 - B200-native decode -> sample -> preprocess -> embed/classify path.
+"""cosmos_curate_b200 - H100-native decode -> sample -> preprocess -> embed/classify path.
 
 Host side mirrors the reference's plugin surface (CuratorStage / ModelInterface); all device work is
-hand-written sm_100a CUDA in libcurate_b200.so, bound with ctypes (cosmos_curate_b200/_lib.py).
+hand-written sm_90a CUDA in libcurate_b200.so, bound with ctypes (cosmos_curate_b200/_lib.py).
 """
 
 __version__ = "0.1.0"

@@ -91,6 +91,7 @@ SIGNATURES = {
     "cb_affine_score": (_i, [_vp, _vp, _vp, _f, _vp, _i, _i, _vp]),
     "cb_mp4_index": (_i, [_vp, _vp, C.c_size_t, C.POINTER(Mp4Info), C.POINTER(C.c_int64), C.POINTER(C.c_uint8), _i]),
     "cb_mp4_cut": (_i, [_vp, _vp, C.c_size_t, _i, _i, _vp, C.c_size_t, C.POINTER(C.c_size_t)]),
+    "cb_nvdec_probe": (_i, [_vp]),
     "cb_decoder_create": (_i, [_vp, C.POINTER(_vp)]),
     "cb_decoder_destroy": (None, [_vp]),
     "cb_decoder_decode": (_i, [_vp, _vp, C.c_size_t, _pi32, _i, C.POINTER(SurfacePool), _pi32, C.POINTER(DecodeStats)]),

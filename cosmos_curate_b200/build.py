@@ -1,4 +1,4 @@
-"""Build libcurate_b200.so in-tree with nvcc for sm_100a (no JIT cache: the .so travels with the tree)."""
+"""Build libcurate_b200.so in-tree with nvcc for sm_90a (no JIT cache: the .so travels with the tree)."""
 
 from __future__ import annotations
 
@@ -14,7 +14,7 @@ LIB = PKG / "libcurate_b200.so"
 STAMP = PKG / ".libcurate_b200.stamp"
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17", "--use_fast_math=false",
+    "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17", "--use_fast_math=false",
     "-Xcompiler", "-fPIC,-O3,-fno-fast-math,-ffp-contract=off", "--expt-relaxed-constexpr",
     "-Xptxas", "-v", "-shared", "-cudart", "shared",
 ]  # fmt: skip
@@ -81,7 +81,7 @@ def build(force: bool = False, verbose: bool = False) -> Path:
 
     with ThreadPoolExecutor(max_workers=min(8, os.cpu_count() or 1)) as tp:
         objs = list(tp.map(compile_one, sources()))
-    cmd = [nvcc, "-shared", "-cudart", "shared", "-gencode", "arch=compute_100a,code=sm_100a", *[str(o) for o in objs], "-o", str(LIB), "-ldl"]
+    cmd = [nvcc, "-shared", "-cudart", "shared", "-gencode", "arch=compute_90a,code=sm_90a", *[str(o) for o in objs], "-o", str(LIB), "-ldl"]
     res = subprocess.run(cmd, capture_output=True, text=True, cwd=str(CSRC))
     logs.append(" ".join(cmd) + "\n" + res.stdout + "\n" + res.stderr)
     (PKG / "build.log").write_text("\n".join(logs))

@@ -109,8 +109,8 @@ int cb_init(int device, cb_ctx** out) {
   if ((e = cudaSetDevice(device)) != cudaSuccess) return cb::fail(nullptr, CB_ERR_CUDA, "cudaSetDevice: %s", cudaGetErrorString(e));
   cudaDeviceProp p;
   if ((e = cudaGetDeviceProperties(&p, device)) != cudaSuccess) return cb::fail(nullptr, CB_ERR_CUDA, "cudaGetDeviceProperties: %s", cudaGetErrorString(e));
-  if (p.major != 10)
-    return cb::fail(nullptr, CB_ERR_UNSUPPORTED, "device %d is sm_%d%d; this library is built for sm_100a (B200) only", device, p.major, p.minor);
+  if (p.major != 9 || p.minor != 0)
+    return cb::fail(nullptr, CB_ERR_UNSUPPORTED, "device %d is sm_%d%d; this library is built for sm_90a (H100) only", device, p.major, p.minor);
   cb_ctx* ctx = new cb_ctx();
   ctx->device = device;
   ctx->sm_count = p.multiProcessorCount;

@@ -1,0 +1,288 @@
+// softmax(Q K^T / sqrt(d)) V on the Hopper tensor cores (wgmma) for the ViT-L/14 shape class: head_dim 64, 129..257 tokens.
+//
+// 257 = 4 * 64 + 1: the first 256 tokens map onto the tensor cores with no padding at all - four 64-row query tiles against
+// one 256-key tile (S = Q K^T is one chain of wgmma m64n256k16 per query tile; no online softmax, every key of the row is in
+// the warpgroup's registers at once).  Token 256 rides along as a ninth..sixteenth of a tile: its key is one more N = 8 product
+// (columns past the first masked), its value one more k-step of P V, and its query row is computed by one SIMT warp.
+// Persistent CTAs (one per SM) loop over (image, head) units; Q, K and V of a unit arrive by TMA into a two-deep ring.
+//
+// Warp roles (384 threads):
+//   warpgroup 0  warp 0: TMA producer (Q 32 KB, K 32 + 1 KB, V 32 + 2 KB per unit from the [n*T][3*hidden] QKV matrix)
+//                warp 1: query row 256 entirely on SIMT (257 dot products of 64 + softmax + 257-term weighted sum from smem K/V)
+//   warpgroups 1-2  query rows 0..127 / 128..255, 64 at a time: S in registers (128 per thread), row max / exp2 / row sum with
+//                quad shuffles, P packed to fp16 IN PLACE as the register A operand of O = P V (the accumulator layout of S is
+//                the A layout of the next product; V is consumed straight from its [key][dim] rows as an MN-major B operand,
+//                no transpose pass), O / rowsum -> fp16 -> global.
+#include <cstdlib>
+#include <cstring>
+
+#include "common.h"
+#include "ptx.cuh"
+
+namespace cb {
+
+constexpr int kAtThreads = 384;
+constexpr int kAtQ = 0;                       // 256 rows x 128 B, SW128
+constexpr int kAtK = 32768;                   // 256 rows, then the 8-row tile that starts at token 256
+constexpr int kAtV = kAtK + 32768 + 1024;     // 256 rows, then the 16-row tile that starts at token 256
+constexpr int kAtStage = kAtV + 32768 + 2048;  // 101376 B: a multiple of 1024
+constexpr int kAtPx = 2 * kAtStage;           // [256] fp32 probabilities of query row 256
+constexpr int kAtBar = kAtPx + 1024;
+constexpr int kAtSmem = kAtBar + 64 + 1024 /* alignment slack */;
+static_assert(kAtStage % 1024 == 0 && kAtSmem <= 232448, "shared memory budget");
+
+struct AttnArgs {
+  const __half* qkv;
+  __half* out;
+  int tokens, heads, n_units;  // n_units = images * heads
+  float scale_log2e;
+};
+
+__device__ __forceinline__ float ex2f(float x) {
+  float y;
+  asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
+  return y;
+}
+__device__ __forceinline__ uint32_t pack2(float a, float b) {
+  __half2 h = __floats2half2_rn(a, b);
+  return *reinterpret_cast<uint32_t*>(&h);
+}
+
+// FULL: tokens is 256 or 257, i.e. every column / row of the tensor-core tiles is a real token (no masking code at all)
+template <bool FULL>
+__global__ void __launch_bounds__(kAtThreads, 1) attention_wgmma_kernel(const __grid_constant__ CUtensorMap map_qkv, const __grid_constant__ CUtensorMap map_k8,
+                                                                         const __grid_constant__ CUtensorMap map_v16, const AttnArgs a) {
+  extern __shared__ __align__(1024) uint8_t smem_raw[];
+  const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;
+  uint8_t* smem = smem_raw + (base - smem_u32(smem_raw));
+  float* px = reinterpret_cast<float*>(smem + kAtPx);
+  uint64_t* full = reinterpret_cast<uint64_t*>(smem + kAtBar);
+  uint64_t* empty = full + 2;
+
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int T = a.tokens, hidden = a.heads * 64;
+  const bool has_extra = T == 257;
+  const int t_mma = FULL ? 256 : (T < 256 ? T : 256);  // keys / query rows living in the tensor-core tiles
+  const size_t row_stride = (size_t)3 * hidden;
+
+  if (threadIdx.x == 0) {
+    tma_prefetch_desc(&map_qkv);
+    for (int i = 0; i < 2; ++i) mbar_init(&full[i], 1), mbar_init(&empty[i], 9);  // 8 consumer warps + the row-256 warp
+    fence_barrier_init();
+  }
+  __syncthreads();
+
+  if (warp < 4) {
+    reg_dealloc<64>();
+    if (warp == 0) {
+      if (lane == 0) {  // ===== TMA producer
+        int it = 0;
+        for (int u = blockIdx.x; u < a.n_units; u += gridDim.x, ++it) {
+          const int img = u / a.heads, h = u - img * a.heads, row0 = img * T, s = it & 1;
+          uint8_t* st = smem + s * kAtStage;
+          mbar_wait_parked(&empty[s], ((it >> 1) & 1) ^ 1);
+          mbar_expect_tx(&full[s], 3 * 32768 + (has_extra ? 1024 + 2048 : 0));
+          for (int half = 0; half < 2; ++half) {
+            tma_load_2d(st + kAtK + half * 16384, &map_qkv, &full[s], hidden + h * 64, row0 + half * 128);
+            tma_load_2d(st + kAtQ + half * 16384, &map_qkv, &full[s], h * 64, row0 + half * 128);
+          }
+          if (has_extra) tma_load_2d(st + kAtK + 32768, &map_k8, &full[s], hidden + h * 64, row0 + 256);
+          for (int half = 0; half < 2; ++half) tma_load_2d(st + kAtV + half * 16384, &map_qkv, &full[s], 2 * hidden + h * 64, row0 + half * 128);
+          if (has_extra) tma_load_2d(st + kAtV + 32768, &map_v16, &full[s], 2 * hidden + h * 64, row0 + 256);
+        }
+      }
+    } else if (warp == 1) {  // ===== query row 256 on SIMT
+      int it = 0;
+      for (int u = blockIdx.x; u < a.n_units; u += gridDim.x, ++it) {
+        const int img = u / a.heads, h = u - img * a.heads, s = it & 1;
+        const size_t row0 = (size_t)img * T;
+        const uint8_t* sK = smem + s * kAtStage + kAtK;
+        const uint8_t* sV = smem + s * kAtStage + kAtV;
+        mbar_wait_parked(&full[s], (it >> 1) & 1);
+        if (has_extra) {
+          const __half* xrow = a.qkv + (row0 + 256) * row_stride + h * 64;
+          auto dot = [&](const uint8_t* krow, int key) {  // rows are 128-byte swizzled: 16-byte unit j of row `key` sits at j ^ (key & 7)
+            float acc = 0.f;
+#pragma unroll
+            for (int j = 0; j < 8; ++j) {
+              const uint4 kb = *reinterpret_cast<const uint4*>(krow + ((j ^ (key & 7)) << 4));
+              const uint4 qj = __ldg(reinterpret_cast<const uint4*>(xrow) + j);  // L1-resident; not kept in registers (this warpgroup runs on 64)
+              const __half2* q2 = reinterpret_cast<const __half2*>(&qj);
+              const __half2* k2 = reinterpret_cast<const __half2*>(&kb);
+#pragma unroll
+              for (int e = 0; e < 4; ++e) {
+                const float2 qf = __half22float2(q2[e]), kf = __half22float2(k2[e]);
+                acc = fmaf(qf.x, kf.x, acc), acc = fmaf(qf.y, kf.y, acc);
+              }
+            }
+            return acc;
+          };
+          float sc[8];
+#pragma unroll
+          for (int i = 0; i < 8; ++i) {
+            const int key = lane + 32 * i;
+            sc[i] = dot(sK + key * 128, key);
+          }
+          const float s_x = dot(sK + 32768, 0);
+          float mx = s_x;
+#pragma unroll
+          for (int i = 0; i < 8; ++i) mx = fmaxf(mx, sc[i]);
+          for (int off = 16; off; off >>= 1) mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, off));
+          const float mb = mx * a.scale_log2e;
+          float sum = 0.f;
+#pragma unroll
+          for (int i = 0; i < 8; ++i) {
+            const float p = ex2f(fmaf(sc[i], a.scale_log2e, -mb));
+            px[lane + 32 * i] = p;
+            sum += p;
+          }
+          for (int off = 16; off; off >>= 1) sum += __shfl_xor_sync(0xffffffffu, sum, off);
+          const float p_x = ex2f(fmaf(s_x, a.scale_log2e, -mb));
+          sum += p_x;
+          __syncwarp();
+          // lane owns output dims 2*lane, 2*lane+1: byte lane*4 of every V row -> 16-byte chunk lane>>2, offset (lane&3)*4
+          const uint8_t* vbase = sV + (lane & 3) * 4;
+          const int ch = lane >> 2;
+          float oa[4] = {0.f, 0.f, 0.f, 0.f}, ob[4] = {0.f, 0.f, 0.f, 0.f};
+#pragma unroll 4
+          for (int key = 0; key < 256; key += 4) {
+            const float4 p4 = *reinterpret_cast<const float4*>(px + key);
+            const float pv[4] = {p4.x, p4.y, p4.z, p4.w};
+#pragma unroll
+            for (int e = 0; e < 4; ++e) {  // four independent accumulator pairs: the loop is not an FMA latency chain
+              const int kk = key + e;
+              const float2 vf = __half22float2(*reinterpret_cast<const __half2*>(vbase + kk * 128 + ((ch ^ (kk & 7)) << 4)));
+              oa[e] = fmaf(pv[e], vf.x, oa[e]), ob[e] = fmaf(pv[e], vf.y, ob[e]);
+            }
+          }
+          float o0 = (oa[0] + oa[1]) + (oa[2] + oa[3]), o1 = (ob[0] + ob[1]) + (ob[2] + ob[3]);
+          const float2 vxf = __half22float2(*reinterpret_cast<const __half2*>(sV + 32768 + lane * 4));  // row 0 of the tile: unswizzled
+          o0 = fmaf(p_x, vxf.x, o0), o1 = fmaf(p_x, vxf.y, o1);
+          const float inv = 1.0f / sum;
+          *reinterpret_cast<uint32_t*>(a.out + (row0 + 256) * hidden + h * 64 + 2 * lane) = pack2(o0 * inv, o1 * inv);
+        }
+        __syncwarp();
+        if (lane == 0) mbar_arrive(&empty[s]);
+      }
+    }
+  } else {  // ===== consumers: warpgroup c owns query rows 128c..128c+127, 64 at a time
+    reg_alloc<216>();
+    const int c = (warp >> 2) - 1, quad = lane & 3;
+    const int r_in = (warp & 3) * 16 + (lane >> 2);  // this thread's first row inside a 64-row tile; the second is r_in + 8
+    int it = 0;
+    for (int u = blockIdx.x; u < a.n_units; u += gridDim.x, ++it) {
+      const int img = u / a.heads, h = u - img * a.heads, s = it & 1;
+      const size_t row0 = (size_t)img * T;
+      const uint32_t st = smem_u32(smem + s * kAtStage);
+      mbar_wait_parked(&full[s], (it >> 1) & 1);
+#pragma unroll 1
+      for (int qt = 0; qt < 2; ++qt) {
+        const int tile_row = c * 128 + qt * 64;
+        if (!FULL && tile_row >= t_mma) break;  // warpgroup-uniform
+        const uint64_t dq = wgmma_desc_sw128(st + kAtQ + tile_row * 128), dk = wgmma_desc_sw128(st + kAtK);
+        float sc[128], sx[4];
+        wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < 4; ++k) wgmma_m64n256k16(sc, dq + (uint64_t)(2 * k), dk + (uint64_t)(2 * k), k != 0);
+        if (has_extra) {
+          const uint64_t dkx = wgmma_desc_sw128(st + kAtK + 32768);
+#pragma unroll
+          for (int k = 0; k < 4; ++k) wgmma_m64n8k16(sx, dq + (uint64_t)(2 * k), dkx + (uint64_t)(2 * k), k != 0);
+        }
+        wgmma_commit();
+        wgmma_wait<0>();
+        // sc[4j + 2h + e] = S(row r_in + 8h, key 8j + 2 quad + e); key 256 of row r_in + 8h is sx[2h] of the quad's first lane
+        const bool own_x = has_extra && quad == 0;
+        float mx[2] = {own_x ? sx[0] : -INFINITY, own_x ? sx[2] : -INFINITY};
+#pragma unroll
+        for (int j = 0; j < 32; ++j)
+#pragma unroll
+          for (int e = 0; e < 4; ++e) {
+            if (!FULL && 8 * j + 2 * quad + (e & 1) >= t_mma) sc[4 * j + e] = -INFINITY;
+            mx[e >> 1] = fmaxf(mx[e >> 1], sc[4 * j + e]);
+          }
+        float mb[2], sum[2], p_x[2];
+#pragma unroll
+        for (int hh = 0; hh < 2; ++hh) {
+          mx[hh] = fmaxf(mx[hh], __shfl_xor_sync(0xffffffffu, mx[hh], 1));
+          mx[hh] = fmaxf(mx[hh], __shfl_xor_sync(0xffffffffu, mx[hh], 2));
+          mb[hh] = mx[hh] * a.scale_log2e;
+          p_x[hh] = own_x ? ex2f(fmaf(sx[2 * hh], a.scale_log2e, -mb[hh])) : 0.f;
+          sum[hh] = p_x[hh];
+        }
+        // P = exp2(S * scale - max) -> fp16 pairs: pa[4ks .. 4ks + 3] is the A fragment of k-step ks (keys 16ks .. 16ks + 15)
+        uint32_t pa[64];
+#pragma unroll
+        for (int j = 0; j < 32; ++j)
+#pragma unroll
+          for (int hh = 0; hh < 2; ++hh) {
+            const float p0 = ex2f(fmaf(sc[4 * j + 2 * hh], a.scale_log2e, -mb[hh])), p1 = ex2f(fmaf(sc[4 * j + 2 * hh + 1], a.scale_log2e, -mb[hh]));
+            sum[hh] += p0 + p1;
+            pa[2 * j + hh] = pack2(p0, p1);
+          }
+        const uint32_t pax[4] = {pack2(p_x[0], 0.f), pack2(p_x[1], 0.f), 0u, 0u};  // key 256, then fifteen zero columns
+        float o[32];
+        wgmma_fence();
+#pragma unroll
+        for (int ks = 0; ks < 16; ++ks) wgmma_m64n64k16_ra_tb(o, pa + 4 * ks, wgmma_desc_sw128_mn(st + kAtV + ks * 2048), ks != 0);
+        if (has_extra) wgmma_m64n64k16_ra_tb(o, pax, wgmma_desc_sw128_mn(st + kAtV + 32768), 1);
+        wgmma_commit();
+        wgmma_wait<0>();
+#pragma unroll
+        for (int i = 0; i < 64; ++i) asm volatile("" ::"r"(pa[i]));  // the A fragments stay in their registers until the MMAs have read them
+#pragma unroll
+        for (int hh = 0; hh < 2; ++hh) {
+          sum[hh] += __shfl_xor_sync(0xffffffffu, sum[hh], 1);
+          sum[hh] += __shfl_xor_sync(0xffffffffu, sum[hh], 2);
+          const int row = tile_row + r_in + 8 * hh;
+          if (!FULL && row >= t_mma) continue;
+          const float inv = 1.0f / sum[hh];
+          __half* orow = a.out + (row0 + row) * hidden + h * 64 + 2 * quad;
+#pragma unroll
+          for (int j = 0; j < 8; ++j) *reinterpret_cast<uint32_t*>(orow + 8 * j) = pack2(o[4 * j + 2 * hh] * inv, o[4 * j + 2 * hh + 1] * inv);
+        }
+      }
+      __syncwarp();
+      if (lane == 0) mbar_arrive(&empty[s]);
+    }
+  }
+}
+
+// host side: launches and sets *launched for the shape class this kernel serves; other shapes go to the mma.sync kernel
+int attention_wgmma(cb_ctx* ctx, const void* qkv, void* out, int n, int tokens, int heads, int head_dim, cudaStream_t stream, bool* launched) {
+  *launched = false;
+  const char* sel = std::getenv("CB_ATTN_KERNEL");
+  if (sel && std::strcmp(sel, "mma") == 0) return CB_OK;
+  if (head_dim != 64 || tokens < 129 || tokens > 257) return CB_OK;
+  const int hidden = heads * 64;
+  CUtensorMap map, map_k8, map_v16;
+  const uint64_t dims[2] = {(uint64_t)3 * hidden, (uint64_t)n * tokens}, strides[1] = {(uint64_t)3 * hidden * 2};
+  const uint32_t box[2] = {64, 128}, box8[2] = {64, 8}, box16[2] = {64, 16};
+  int rc = make_tensor_map(ctx, &map, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, qkv, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_128B);
+  if (rc) return rc;
+  // the tiles that start at token 256: one MMA n-step of keys, one MMA k-step of values.  Their rows past token 256 belong to the
+  // next image (or are zero-filled past the end of the matrix); the kernel gives them zero probability.
+  rc = make_tensor_map(ctx, &map_k8, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, qkv, dims, strides, box8, CU_TENSOR_MAP_SWIZZLE_128B);
+  if (rc) return rc;
+  rc = make_tensor_map(ctx, &map_v16, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, qkv, dims, strides, box16, CU_TENSOR_MAP_SWIZZLE_128B);
+  if (rc) return rc;
+  static bool attr_done[64] = {};  // the attribute is per device: one process may drive several
+  bool& attr_set = attr_done[ctx->device & 63];
+  if (!attr_set) {
+    CB_CUDA(ctx, cudaFuncSetAttribute(attention_wgmma_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kAtSmem));
+    CB_CUDA(ctx, cudaFuncSetAttribute(attention_wgmma_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kAtSmem));
+    attr_set = true;
+  }
+  AttnArgs a{(const __half*)qkv, (__half*)out, tokens, heads, n * heads, 1.4426950408889634f / sqrtf(64.f)};
+  const int grid = std::min(n * heads, ctx->sm_count);
+  mark_launch(ctx, CB_PROF_ATTENTION, stream);
+  if (tokens >= 256)
+    attention_wgmma_kernel<true><<<grid, kAtThreads, kAtSmem, stream>>>(map, map_k8, map_v16, a);
+  else
+    attention_wgmma_kernel<false><<<grid, kAtThreads, kAtSmem, stream>>>(map, map_k8, map_v16, a);
+  CB_CUDA(ctx, cudaGetLastError());
+  *launched = true;
+  return CB_OK;
+}
+
+}  // namespace cb

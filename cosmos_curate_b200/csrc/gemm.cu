@@ -1,14 +1,13 @@
-// tcgen05 GEMM for the image tower (sm_100a):  C[M][N] = epilogue(A[M][K] . W[N][K]^T + bias) (+ residual)
+// wgmma GEMM for the image tower (sm_90a):  C[M][N] = epilogue(A[M][K] . W[N][K]^T + bias) (+ residual)
 //
-//  * fp16 operands, fp32 accumulation in TMEM; one 128 x BN output tile per CTA iteration, persistent
-//    grid (one CTA per SM) walking tiles n-fastest so the A row-block stays in L2 while W streams.
-//  * warp 0: TMA producer (cp.async.bulk.tensor 2-D, 128-byte swizzle, kStages-deep mbarrier ring)
-//    warp 1: MMA issuer (one thread, tcgen05.mma.cta_group::1.kind::f16, UMMA 128 x BN x 16)
-//    warp 2: TMEM allocator (2 accumulator buffers of BN fp32 columns -> MMA of tile i+1 overlaps the
-//            epilogue of tile i)
-//    warps 4-7: epilogue (tcgen05.ld 32x32b.x32 -> bias / activation / residual -> 128-bit stores)
-//  * Every Linear of HF CLIPEncoderLayer / SiglipEncoderLayer (q,k,v fused; out_proj; fc1; fc2) and the
-//    patch-embed conv (im2col rows produced by the preprocess kernel) go through this kernel.
+//  * fp16 operands, fp32 accumulation in registers; one 128 x BN output tile per CTA iteration, persistent grid (one CTA
+//    per SM) walking tiles n-fastest so the A row-block stays in L2 while W streams.
+//  * warpgroup 0: warp 0 is the TMA producer (cp.async.bulk.tensor 2-D, 128-byte swizzle, kStages-deep mbarrier ring); the
+//    group gives its registers away (setmaxnreg).
+//    warpgroups 1-2: consumers; each owns 64 rows of the tile (wgmma m64 x BN x k16, both operands from shared memory), keeps
+//    one k-block of MMAs in flight and runs the epilogue (bias / activation / residual) from its accumulator registers.
+//  * Every Linear of HF CLIPEncoderLayer / SiglipEncoderLayer (q,k,v fused; out_proj; fc1; fc2) and the patch-embed conv
+//    (im2col rows produced by the preprocess kernel) go through this kernel.
 #include <cuda_fp16.h>
 
 #include <algorithm>
@@ -20,7 +19,7 @@
 namespace cb {
 
 constexpr int BM = 128, BK = 64;
-constexpr int kGemmThreads = 256;
+constexpr int kGemmThreads = 384;
 
 template <int BN>
 struct GemmCfg {
@@ -28,7 +27,6 @@ struct GemmCfg {
   static constexpr int kABytes = BM * BK * 2, kBBytes = BN * BK * 2;
   static constexpr int kStageBytes = kABytes + kBBytes;
   static constexpr int kSmem = kStages * kStageBytes + 1024 /*align slack*/ + 256 /*barriers*/;
-  static constexpr int kTmemCols = 2 * BN;  // 512 (BN=256) or 256 (BN=128): powers of two
 };
 
 struct GemmArgs {
@@ -49,115 +47,55 @@ __device__ __forceinline__ float act_gelu_tanh(float x) {
   return 0.5f * x * (1.f + t);
 }
 
-// One 32-column chunk of the epilogue for this thread's output row: TMEM -> registers -> bias / activation /
-// residual -> 128-bit global stores.
-template <int ACT, bool OUT_F32>
-__device__ __forceinline__ void epilogue_chunk(const GemmArgs& g, uint32_t taddr, int row, bool row_ok, int col0) {
-  uint32_t r[32];
-  tmem_ld_32x32b_x32(taddr, r);
-  tmem_ld_wait();
-  float v[32];
-#pragma unroll
-  for (int j = 0; j < 32; ++j) v[j] = __uint_as_float(r[j]);
-  if (g.bias) {
-#pragma unroll
-    for (int j4 = 0; j4 < 8; ++j4) {
-      if (col0 + j4 * 4 < g.N) {
-        const float4 b = __ldg((const float4*)(g.bias + col0) + j4);
-        v[j4 * 4 + 0] += b.x, v[j4 * 4 + 1] += b.y, v[j4 * 4 + 2] += b.z, v[j4 * 4 + 3] += b.w;
-      }
-    }
-  }
-  if (ACT == CB_EPI_QUICK_GELU) {
-#pragma unroll
-    for (int j = 0; j < 32; ++j) v[j] = act_quick_gelu(v[j]);
-  } else if (ACT == CB_EPI_GELU_TANH) {
-#pragma unroll
-    for (int j = 0; j < 32; ++j) v[j] = act_gelu_tanh(v[j]);
-  }
-  if (!row_ok) return;
-  if (OUT_F32) {
-    float4* dst = (float4*)(g.out_f32 + (size_t)row * g.N + col0);
-    const float4* res = g.residual ? (const float4*)(g.residual + (size_t)row * g.N + col0) : nullptr;
-#pragma unroll
-    for (int j4 = 0; j4 < 8; ++j4) {
-      if (col0 + j4 * 4 < g.N) {
-        float4 o = make_float4(v[j4 * 4], v[j4 * 4 + 1], v[j4 * 4 + 2], v[j4 * 4 + 3]);
-        if (res) {
-          const float4 rr = res[j4];
-          o.x += rr.x, o.y += rr.y, o.z += rr.z, o.w += rr.w;
-        }
-        dst[j4] = o;
-      }
-    }
-  } else {
-    uint4* dst = (uint4*)(g.out_f16 + (size_t)row * g.N + col0);
-#pragma unroll
-    for (int j8 = 0; j8 < 4; ++j8) {
-      if (col0 + j8 * 8 < g.N) {
-        __half2 h0 = __floats2half2_rn(v[j8 * 8 + 0], v[j8 * 8 + 1]);
-        __half2 h1 = __floats2half2_rn(v[j8 * 8 + 2], v[j8 * 8 + 3]);
-        __half2 h2 = __floats2half2_rn(v[j8 * 8 + 4], v[j8 * 8 + 5]);
-        __half2 h3 = __floats2half2_rn(v[j8 * 8 + 6], v[j8 * 8 + 7]);
-        uint4 o;
-        o.x = *(uint32_t*)&h0, o.y = *(uint32_t*)&h1, o.z = *(uint32_t*)&h2, o.w = *(uint32_t*)&h3;
-        dst[j8] = o;
-      }
-    }
-  }
+template <int ACT>
+__device__ __forceinline__ float act(float x) {
+  if (ACT == CB_EPI_QUICK_GELU) return act_quick_gelu(x);
+  if (ACT == CB_EPI_GELU_TANH) return act_gelu_tanh(x);
+  return x;
+}
+
+template <int BN>
+__device__ __forceinline__ void wgmma_tile(float* d, uint64_t da, uint64_t db, int accumulate) {
+  if (BN == 256) wgmma_m64n256k16(d, da, db, accumulate);
+  else wgmma_m64n128k16(d, da, db, accumulate);
 }
 
 template <int BN, int ACT, bool OUT_F32>
 __global__ void __launch_bounds__(kGemmThreads, 1)
-    gemm_tcgen05_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b, const GemmArgs g) {
+    gemm_wgmma_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b, const GemmArgs g) {
   using Cfg = GemmCfg<BN>;
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;
   uint8_t* smem = smem_raw + (base - smem_u32(smem_raw));
-  uint8_t* sA = smem;                                    // [stages][128][64] fp16, SW128
-  uint8_t* sB = smem + Cfg::kStages * Cfg::kABytes;      // [stages][BN][64]
-  uint64_t* bars = (uint64_t*)(smem + Cfg::kStages * Cfg::kStageBytes);
-  uint64_t* full = bars;
-  uint64_t* empty = bars + Cfg::kStages;
-  uint64_t* tfull = bars + 2 * Cfg::kStages;
-  uint64_t* tempty = tfull + 2;
-  uint32_t* tmem_slot = (uint32_t*)(tempty + 2);
+  uint8_t* sA = smem;                                // [stages][128][64] fp16, SW128
+  uint8_t* sB = smem + Cfg::kStages * Cfg::kABytes;  // [stages][BN][64]
+  uint64_t* full = (uint64_t*)(smem + Cfg::kStages * Cfg::kStageBytes);
+  uint64_t* empty = full + Cfg::kStages;
 
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, wg = warp >> 2;
   const int m_tiles = (g.M + BM - 1) / BM, n_tiles = (g.N + BN - 1) / BN;
   const int num_tiles = m_tiles * n_tiles;
   const int num_kb = (g.K + BK - 1) / BK;
+  const int first = blockIdx.x, step = gridDim.x;
 
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 0) {
     tma_prefetch_desc(&map_a);
     tma_prefetch_desc(&map_b);
-  }
-  if (warp == 1 && lane == 0) {
     for (int i = 0; i < Cfg::kStages; ++i) {
       mbar_init(&full[i], 1);
-      mbar_init(&empty[i], 1);
-    }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&tfull[i], 1);
-      mbar_init(&tempty[i], 4);  // one arrival per epilogue warp
+      mbar_init(&empty[i], 2);  // one arrival per consumer warpgroup
     }
     fence_barrier_init();
   }
-  if (warp == 2) {
-    tmem_alloc(tmem_slot, Cfg::kTmemCols);
-    tmem_relinquish();
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
-  if (warp == 0) {
-    if (lane == 0) {  // ===== TMA producer
+  if (wg == 0) {
+    reg_dealloc<40>();
+    if (warp == 0 && lane == 0) {  // ===== TMA producer
       int stage = 0;
       uint32_t phase = 0;
-      for (int t = blockIdx.x; t < num_tiles; t += gridDim.x) {
-        const int m_blk = t / n_tiles, n_blk = t - m_blk * n_tiles;
+      for (int t = first; t < num_tiles; t += step) {
+        const int m_blk = t / n_tiles, n_blk = t % n_tiles;
         for (int kb = 0; kb < num_kb; ++kb) {
           mbar_wait(&empty[stage], phase ^ 1);
           mbar_expect_tx(&full[stage], Cfg::kStageBytes);
@@ -167,279 +105,67 @@ __global__ void __launch_bounds__(kGemmThreads, 1)
         }
       }
     }
-  } else if (warp == 1) {
-    if (lane == 0) {  // ===== MMA issuer
-      constexpr uint32_t idesc = umma_idesc_f16(BM, BN, 0);
-      int stage = 0, acc = 0;
-      uint32_t phase = 0, acc_phase = 0;
-      for (int t = blockIdx.x; t < num_tiles; t += gridDim.x) {
-        mbar_wait(&tempty[acc], acc_phase ^ 1);
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + (uint32_t)(acc * BN);
-        for (int kb = 0; kb < num_kb; ++kb) {
-          mbar_wait(&full[stage], phase);
-          tc_fence_after();
-          const uint64_t da = umma_desc_sw128(smem_u32(sA + stage * Cfg::kABytes));
-          const uint64_t db = umma_desc_sw128(smem_u32(sB + stage * Cfg::kBBytes));
+  } else {  // ===== consumers: warpgroup c owns rows 64c..64c+63 of the tile
+    reg_alloc<232>();
+    const int c = wg - 1;
+    auto release = [&](int s) {  // this warpgroup's MMAs have finished reading slot s
+      if ((threadIdx.x & 127) == 0) mbar_arrive(&empty[s]);
+    };
+    int stage = 0;
+    uint32_t phase = 0;
+    float acc[BN / 2];
+    for (int t = first; t < num_tiles; t += step) {
+      const int m_blk = t / n_tiles, n_blk = t % n_tiles;
+      int prev = -1;
+      for (int kb = 0; kb < num_kb; ++kb) {
+        mbar_wait(&full[stage], phase);
+        const uint64_t da = wgmma_desc_sw128(smem_u32(sA + stage * Cfg::kABytes + c * (64 * 128)));
+        const uint64_t db = wgmma_desc_sw128(smem_u32(sB + stage * Cfg::kBBytes));
+        wgmma_fence();
 #pragma unroll
-          for (int k = 0; k < BK / 16; ++k)  // +32 bytes (>>4 = 2) per UMMA_K inside the 128-byte swizzle atom
-            umma_f16(d_tmem, da + (uint64_t)(2 * k), db + (uint64_t)(2 * k), idesc, (kb | k) != 0);
-          umma_commit(&empty[stage]);  // smem slot reusable once these MMAs have read it
-          if (++stage == Cfg::kStages) stage = 0, phase ^= 1;
-        }
-        umma_commit(&tfull[acc]);  // accumulator complete
-        if ((acc ^= 1) == 0) acc_phase ^= 1;
+        for (int k = 0; k < BK / 16; ++k) wgmma_tile<BN>(acc, da + (uint64_t)(2 * k), db + (uint64_t)(2 * k), (kb | k) != 0);
+        wgmma_commit();
+        wgmma_wait<1>();  // the previous k-block's MMAs are complete: its slot may be refilled
+        if (prev >= 0) release(prev);
+        prev = stage;
+        if (++stage == Cfg::kStages) stage = 0, phase ^= 1;
       }
-    }
-  } else if (warp >= 4) {  // ===== epilogue: warp q owns TMEM lanes [32q, 32q+32)
-    const int q = warp & 3;
-    int acc = 0;
-    uint32_t acc_phase = 0;
-    for (int t = blockIdx.x; t < num_tiles; t += gridDim.x) {
-      const int m_blk = t / n_tiles, n_blk = t - m_blk * n_tiles;
-      mbar_wait(&tfull[acc], acc_phase);
-      tc_fence_after();
-      const int row = m_blk * BM + q * 32 + lane;
-      const bool row_ok = row < g.M;
-#pragma unroll 1
-      for (int cc = 0; cc < BN / 32; ++cc) {
-        const int col0 = n_blk * BN + cc * 32;
-        if (col0 >= g.N) break;  // warp-uniform
-        epilogue_chunk<ACT, OUT_F32>(g, tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(acc * BN + cc * 32), row, row_ok, col0);
-      }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&tempty[acc]);
-      if ((acc ^= 1) == 0) acc_phase ^= 1;
-    }
-  }
+      wgmma_wait<0>();
+      release(prev);
 
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 2) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, Cfg::kTmemCols);
-  }
-}
-
-
-// ================================================================================================ 2-CTA kernel
-// A CTA pair (cluster of 2 on one TPC) owns a 256 x 256 output tile: tcgen05.mma.cta_group::2 with UMMA_M = 256.
-// Each CTA stages its own 128 rows of A and ONE HALF (128 rows) of the W tile; the MMA reads W from both CTAs'
-// shared memory, so per-CTA L2 traffic per k-block drops from 48 KB (1-CTA 128x256) to 32 KB and the flop/byte of the
-// tile rises from 85 to 131 - the 1-CTA kernel measured L2-bound at ~12 TB/s.  Roles per CTA:
-//   warp 0 TMA producer (loads credited to the LEADER's full barrier), warp 1 MMA issuer (leader CTA only),
-//   warp 2 TMEM allocator, warps 4-11 epilogue (two warps per TMEM lane quarter, each half of the columns).
-constexpr int kGemm2Threads = 384;
-constexpr int BN2 = 256;
-
-struct Gemm2Cfg {
-  static constexpr int kStages = 5;
-  static constexpr int kABytes = BM * BK * 2, kBBytes = (BN2 / 2) * BK * 2;
-  static constexpr int kStageBytes = kABytes + kBBytes;  // per CTA
-  static constexpr int kEpiBytes = 8 * 4096;             // one 32x32 fp32 staging tile per epilogue warp (TMA store / reduce-add)
-  static constexpr int kSmem = kStages * kStageBytes + kEpiBytes + 1024 + 256;
-  static constexpr int kTmemCols = 2 * BN2;
-};
-
-// EPI_TMA (fp32 output only): the epilogue stages each 32x32 chunk in shared memory (128-byte swizzle) and hands it to the
-// TMA: plain store, or - for the residual stream, out == residual - cp.reduce.async.bulk.tensor .add, i.e. h += tile is
-// performed at L2.  The SMs never read the residual and every global access is a full 128-byte line; the row-per-thread
-// ld/st path it replaces touched 32 lines per instruction and held the K=1024 out-projection at 26 % tensor-pipe activity.
-template <int ACT, bool OUT_F32, bool EPI_TMA>
-__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(kGemm2Threads, 1)
-    gemm_tcgen05_2cta_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b,
-                             const __grid_constant__ CUtensorMap map_c, const GemmArgs g) {
-  using Cfg = Gemm2Cfg;
-  extern __shared__ __align__(1024) uint8_t smem_raw[];
-  const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;
-  uint8_t* smem = smem_raw + (base - smem_u32(smem_raw));
-  uint8_t* sA = smem;
-  uint8_t* sB = smem + Cfg::kStages * Cfg::kABytes;
-  uint8_t* sEpi = smem + Cfg::kStages * Cfg::kStageBytes;  // 1024-byte aligned: stage sizes are multiples of 1024
-  uint64_t* bars = (uint64_t*)(sEpi + Cfg::kEpiBytes);
-  uint64_t* full = bars;
-  uint64_t* empty = bars + Cfg::kStages;
-  uint64_t* tfull = bars + 2 * Cfg::kStages;
-  uint64_t* tempty = tfull + 2;
-  uint32_t* tmem_slot = (uint32_t*)(tempty + 2);
-
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const uint32_t rank = cluster_ctarank();
-  const bool leader = rank == 0;
-  const int m_tiles = (g.M + 2 * BM - 1) / (2 * BM), n_tiles = (g.N + BN2 - 1) / BN2;
-  const int num_tiles = m_tiles * n_tiles;
-  const int num_kb = (g.K + BK - 1) / BK;
-  const int pair = blockIdx.x >> 1, num_pairs = gridDim.x >> 1;
-
-  if (warp == 0 && lane == 0) {
-    tma_prefetch_desc(&map_a);
-    tma_prefetch_desc(&map_b);
-  }
-  if (warp == 1 && lane == 0) {
-    for (int i = 0; i < Cfg::kStages; ++i) {
-      mbar_init(&full[i], 1);   // leader: its own arrive.expect_tx for the bytes of BOTH CTAs
-      mbar_init(&empty[i], 1);  // multicast tcgen05.commit arrives in both CTAs
-    }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&tfull[i], 1);
-      mbar_init(&tempty[i], 16);  // 8 epilogue warps of each CTA arrive on the leader's copy
-    }
-    fence_barrier_init();
-  }
-  if (warp == 2) {
-    tmem_alloc_2cta(tmem_slot, Cfg::kTmemCols);
-    tmem_relinquish_2cta();
-  }
-  tc_fence_before();
-  cluster_sync_all();  // barriers of both CTAs are initialised before any remote arrive / TMA completion
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-
-  if (warp == 0) {
-    if (lane == 0) {  // ===== TMA producer (both CTAs)
-      int stage = 0;
-      uint32_t phase = 0;
-      for (int t = pair; t < num_tiles; t += num_pairs) {
-        const int m_blk = t / n_tiles, n_blk = t - m_blk * n_tiles;
-        const int row_a = m_blk * 2 * BM + (int)rank * BM, row_b = n_blk * BN2 + (int)rank * (BN2 / 2);
-        for (int kb = 0; kb < num_kb; ++kb) {
-          mbar_wait(&empty[stage], phase ^ 1);
-          if (leader) mbar_expect_tx(&full[stage], 2 * Cfg::kStageBytes);
-          tma_load_2d_2cta(sA + stage * Cfg::kABytes, &map_a, &full[stage], kb * BK, row_a);
-          tma_load_2d_2cta(sB + stage * Cfg::kBBytes, &map_b, &full[stage], kb * BK, row_b);
-          if (++stage == Cfg::kStages) stage = 0, phase ^= 1;
-        }
-      }
-    }
-  } else if (warp == 1) {
-    if (leader && lane == 0) {  // ===== MMA issuer (leader CTA, one thread)
-      constexpr uint32_t idesc = umma_idesc_f16(2 * BM, BN2, 0);
-      int stage = 0, acc = 0;
-      uint32_t phase = 0, acc_phase = 0;
-      for (int t = pair; t < num_tiles; t += num_pairs) {
-        mbar_wait(&tempty[acc], acc_phase ^ 1);
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + (uint32_t)(acc * BN2);
-        for (int kb = 0; kb < num_kb; ++kb) {
-          mbar_wait(&full[stage], phase);
-          tc_fence_after();
-          const uint64_t da = umma_desc_sw128(smem_u32(sA + stage * Cfg::kABytes));
-          const uint64_t db = umma_desc_sw128(smem_u32(sB + stage * Cfg::kBBytes));
+      // epilogue from registers: acc[4j + 0..1] = (row r0, columns 8j + 2(lane%4) + 0..1), acc[4j + 2..3] = row r0 + 8
+      const int r0 = m_blk * BM + c * 64 + (warp & 3) * 16 + (lane >> 2);
+      const int col_base = n_blk * BN + 2 * (lane & 3);
 #pragma unroll
-          for (int k = 0; k < BK / 16; ++k) umma_f16_2cta(d_tmem, da + (uint64_t)(2 * k), db + (uint64_t)(2 * k), idesc, (kb | k) != 0);
-          umma_commit_2cta(&empty[stage]);
-          if (++stage == Cfg::kStages) stage = 0, phase ^= 1;
-        }
-        umma_commit_2cta(&tfull[acc]);
-        if ((acc ^= 1) == 0) acc_phase ^= 1;
-      }
-    }
-  } else if (warp >= 4) {  // ===== epilogue: lane quarter q, column half `half`
-    const int q = warp & 3, half = (warp - 4) >> 2;
-    uint8_t* stage_buf = sEpi + (warp - 4) * 4096;
-    int acc = 0;
-    uint32_t acc_phase = 0;
-    for (int t = pair; t < num_tiles; t += num_pairs) {
-      const int m_blk = t / n_tiles, n_blk = t - m_blk * n_tiles;
-      mbar_wait(&tfull[acc], acc_phase);
-      tc_fence_after();
-      const int row_base = m_blk * 2 * BM + (int)rank * BM + q * 32;
-      const int row = row_base + lane;
-      const bool row_ok = row < g.M;
-#pragma unroll 1
-      for (int cc = half * (BN2 / 64); cc < (half + 1) * (BN2 / 64); ++cc) {
-        const int col0 = n_blk * BN2 + cc * 32;
-        if (col0 >= g.N) break;  // warp-uniform
-        const uint32_t taddr = tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(acc * BN2 + cc * 32);
-        if (EPI_TMA) {
-          uint32_t r[32];
-          tmem_ld_32x32b_x32(taddr, r);
-          tmem_ld_wait();
-          float v[32];
+      for (int j = 0; j < BN / 8; ++j) {
+        const int col = col_base + 8 * j;
+        if (col >= g.N) break;  // N is a multiple of 8: a column pair is inside or outside as a whole
+        float2 b = make_float2(0.f, 0.f);
+        if (g.bias) b = __ldg((const float2*)(g.bias + col));
 #pragma unroll
-          for (int j = 0; j < 32; ++j) v[j] = __uint_as_float(r[j]);
-          if (g.bias) {
-#pragma unroll
-            for (int j4 = 0; j4 < 8; ++j4) {
-              if (col0 + j4 * 4 < g.N) {
-                const float4 b = __ldg((const float4*)(g.bias + col0) + j4);
-                v[j4 * 4 + 0] += b.x, v[j4 * 4 + 1] += b.y, v[j4 * 4 + 2] += b.z, v[j4 * 4 + 3] += b.w;
-              }
+        for (int h = 0; h < 2; ++h) {
+          const int row = r0 + 8 * h;
+          if (row >= g.M) continue;
+          float v0 = act<ACT>(acc[4 * j + 2 * h] + b.x), v1 = act<ACT>(acc[4 * j + 2 * h + 1] + b.y);
+          if (OUT_F32) {
+            if (g.residual) {
+              const float2 rr = *(const float2*)(g.residual + (size_t)row * g.N + col);
+              v0 += rr.x, v1 += rr.y;
             }
+            *(float2*)(g.out_f32 + (size_t)row * g.N + col) = make_float2(v0, v1);
+          } else {
+            *(__half2*)(g.out_f16 + (size_t)row * g.N + col) = __floats2half2_rn(v0, v1);
           }
-          if (ACT == CB_EPI_QUICK_GELU) {
-#pragma unroll
-            for (int j = 0; j < 32; ++j) v[j] = act_quick_gelu(v[j]);
-          } else if (ACT == CB_EPI_GELU_TANH) {
-#pragma unroll
-            for (int j = 0; j < 32; ++j) v[j] = act_gelu_tanh(v[j]);
-          }
-          if (lane == 0) bulk_wait_read0();  // the previous chunk's TMA has finished reading the staging tile
-          __syncwarp();
-          if (OUT_F32) {  // 32 rows x 128 B, 128-byte swizzle: conflict-free STS.128
-#pragma unroll
-            for (int j4 = 0; j4 < 8; ++j4)
-              *(float4*)(stage_buf + lane * 128 + ((j4 ^ (lane & 7)) << 4)) = make_float4(v[4 * j4], v[4 * j4 + 1], v[4 * j4 + 2], v[4 * j4 + 3]);
-          } else {  // 32 rows x 64 B fp16, 64-byte swizzle
-#pragma unroll
-            for (int j8 = 0; j8 < 4; ++j8) {
-              const __half2 h0 = __floats2half2_rn(v[j8 * 8 + 0], v[j8 * 8 + 1]), h1 = __floats2half2_rn(v[j8 * 8 + 2], v[j8 * 8 + 3]);
-              const __half2 h2 = __floats2half2_rn(v[j8 * 8 + 4], v[j8 * 8 + 5]), h3 = __floats2half2_rn(v[j8 * 8 + 6], v[j8 * 8 + 7]);
-              uint4 o;
-              o.x = *(const uint32_t*)&h0, o.y = *(const uint32_t*)&h1, o.z = *(const uint32_t*)&h2, o.w = *(const uint32_t*)&h3;
-              *(uint4*)(stage_buf + lane * 64 + ((j8 ^ ((lane >> 1) & 3)) << 4)) = o;
-            }
-          }
-          fence_proxy_async();
-          __syncwarp();
-          if (lane == 0) {
-            if (OUT_F32 && g.residual) tma_reduce_add_2d(&map_c, stage_buf, col0, row_base);
-            else tma_store_2d(&map_c, stage_buf, col0, row_base);
-            bulk_commit();
-          }
-        } else {
-          epilogue_chunk<ACT, OUT_F32>(g, taddr, row, row_ok, col0);
         }
       }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive_cluster(map_to_cta(&tempty[acc], 0));  // the leader's MMA thread waits for both CTAs
-      if ((acc ^= 1) == 0) acc_phase ^= 1;
     }
   }
-
-  if (EPI_TMA && warp >= 4 && lane == 0) bulk_wait0();  // outstanding TMA stores / reductions of this warp are complete
-  tc_fence_before();
-  cluster_sync_all();  // the peer's MMAs / epilogue reads of our shared memory and TMEM are complete
-  if (warp == 2) {
-    tc_fence_after();
-    tmem_dealloc_2cta(tmem_base, Cfg::kTmemCols);
-  }
-}
-
-template <int ACT, bool OUT_F32, bool EPI_TMA>
-static int launch_gemm_2cta(cb_ctx* ctx, const CUtensorMap& ma, const CUtensorMap& mb, const CUtensorMap& mc, const GemmArgs& g,
-                            cudaStream_t stream) {
-  auto kern = gemm_tcgen05_2cta_kernel<ACT, OUT_F32, EPI_TMA>;
-  static bool attr_done[64] = {};  // per template instantiation AND per device
-  bool& attr_set = attr_done[ctx->device & 63];
-  if (!attr_set) {
-    CB_CUDA(ctx, cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Gemm2Cfg::kSmem));
-    attr_set = true;
-  }
-  const int tiles = ((g.M + 2 * BM - 1) / (2 * BM)) * ((g.N + BN2 - 1) / BN2);
-  const int pairs = std::min(tiles, ctx->sm_count / 2);
-  mark_launch(ctx, CB_PROF_GEMM, stream);
-  kern<<<2 * pairs, kGemm2Threads, Gemm2Cfg::kSmem, stream>>>(ma, mb, mc, g);
-  CB_CUDA(ctx, cudaGetLastError());
-  return CB_OK;
 }
 
 template <int BN, int ACT, bool OUT_F32>
 static int launch_gemm(cb_ctx* ctx, const CUtensorMap& ma, const CUtensorMap& mb, const GemmArgs& g, cudaStream_t stream) {
   using Cfg = GemmCfg<BN>;
-  auto kern = gemm_tcgen05_kernel<BN, ACT, OUT_F32>;
+  auto kern = gemm_wgmma_kernel<BN, ACT, OUT_F32>;
   static bool attr_done[64] = {};  // per template instantiation AND per device
   bool& attr_set = attr_done[ctx->device & 63];
   if (!attr_set) {
@@ -447,11 +173,19 @@ static int launch_gemm(cb_ctx* ctx, const CUtensorMap& ma, const CUtensorMap& mb
     attr_set = true;
   }
   const int tiles = ((g.M + BM - 1) / BM) * ((g.N + BN - 1) / BN);
-  const int grid = tiles < ctx->sm_count ? tiles : ctx->sm_count;
   mark_launch(ctx, CB_PROF_GEMM, stream);
-  kern<<<grid, kGemmThreads, Cfg::kSmem, stream>>>(ma, mb, g);
+  kern<<<std::min(tiles, ctx->sm_count), kGemmThreads, Cfg::kSmem, stream>>>(ma, mb, g);
   CB_CUDA(ctx, cudaGetLastError());
   return CB_OK;
+}
+
+template <int BN>
+static int dispatch_gemm(cb_ctx* ctx, const CUtensorMap& ma, const CUtensorMap& mb, const GemmArgs& g, int epilogue, cudaStream_t stream) {
+  if (g.out_f32) return launch_gemm<BN, CB_EPI_NONE, true>(ctx, ma, mb, g, stream);
+  if (epilogue == CB_EPI_QUICK_GELU) return launch_gemm<BN, CB_EPI_QUICK_GELU, false>(ctx, ma, mb, g, stream);
+  if (epilogue == CB_EPI_GELU_TANH) return launch_gemm<BN, CB_EPI_GELU_TANH, false>(ctx, ma, mb, g, stream);
+  if (epilogue == CB_EPI_NONE) return launch_gemm<BN, CB_EPI_NONE, false>(ctx, ma, mb, g, stream);
+  return fail(ctx, CB_ERR_ARG, "gemm: unknown epilogue %d", epilogue);
 }
 
 int gemm_f16(cb_ctx* ctx, const void* A, const void* W, const float* bias, const float* residual, float* out_f32, void* out_f16, int M,
@@ -466,47 +200,6 @@ int gemm_f16(cb_ctx* ctx, const void* A, const void* W, const float* bias, const
   const int tiles256 = ((M + BM - 1) / BM) * ((N + 255) / 256);
   const bool wide = (N % 256 == 0 || N > 1024) && tiles256 >= ctx->sm_count;
   const int BN = wide ? 256 : 128;
-  const char* force = getenv("CB_GEMM_KERNEL");  // "1cta" / "2cta": test and A/B switch
-  const int tiles2 = ((M + 255) / 256) * ((N + 255) / 256);
-  bool use2 = tiles2 >= ctx->sm_count / 2 && N >= 256;
-  if (force && force[0] == '1') use2 = false;
-  if (force && force[0] == '2') use2 = true;
-  if (use2) {
-    CUtensorMap ma2, mb2;
-    uint64_t da2[2] = {(uint64_t)K, (uint64_t)M}, db2[2] = {(uint64_t)K, (uint64_t)N}, st2[1] = {(uint64_t)K * 2};
-    uint32_t ba2[2] = {BK, BM}, bb2[2] = {BK, BN2 / 2};
-    int rc2 = make_tensor_map(ctx, &ma2, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, A, da2, st2, ba2, CU_TENSOR_MAP_SWIZZLE_128B);
-    if (rc2) return rc2;
-    rc2 = make_tensor_map(ctx, &mb2, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, W, db2, st2, bb2, CU_TENSOR_MAP_SWIZZLE_128B);
-    if (rc2) return rc2;
-    GemmArgs g2{bias, residual, out_f32, (__half*)out_f16, M, N, K};
-    const char* epi = getenv("CB_GEMM_EPILOGUE");  // "direct": A/B switch for the TMA epilogue
-    const bool tma_ok = !(epi && epi[0] == 'd');
-    if (tma_ok && out_f32 && (residual == nullptr || residual == out_f32) && !((uintptr_t)out_f32 & 15)) {
-      CUtensorMap mc2;
-      uint64_t dc2[2] = {(uint64_t)N, (uint64_t)M}, sc2[1] = {(uint64_t)N * 4};
-      uint32_t bc2[2] = {32, 32};
-      rc2 = make_tensor_map(ctx, &mc2, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, out_f32, dc2, sc2, bc2, CU_TENSOR_MAP_SWIZZLE_128B);
-      if (rc2) return rc2;
-      return launch_gemm_2cta<CB_EPI_NONE, true, true>(ctx, ma2, mb2, mc2, g2, stream);
-    }
-    if (tma_ok && !out_f32 && !((uintptr_t)out_f16 & 15)) {
-      CUtensorMap mc2;
-      uint64_t dc2[2] = {(uint64_t)N, (uint64_t)M}, sc2[1] = {(uint64_t)N * 2};
-      uint32_t bc2[2] = {32, 32};
-      rc2 = make_tensor_map(ctx, &mc2, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, out_f16, dc2, sc2, bc2, CU_TENSOR_MAP_SWIZZLE_64B);
-      if (rc2) return rc2;
-      if (epilogue == CB_EPI_QUICK_GELU) return launch_gemm_2cta<CB_EPI_QUICK_GELU, false, true>(ctx, ma2, mb2, mc2, g2, stream);
-      if (epilogue == CB_EPI_GELU_TANH) return launch_gemm_2cta<CB_EPI_GELU_TANH, false, true>(ctx, ma2, mb2, mc2, g2, stream);
-      if (epilogue == CB_EPI_NONE) return launch_gemm_2cta<CB_EPI_NONE, false, true>(ctx, ma2, mb2, mc2, g2, stream);
-      return fail(ctx, CB_ERR_ARG, "gemm: unknown epilogue %d", epilogue);
-    }
-    if (out_f32) return launch_gemm_2cta<CB_EPI_NONE, true, false>(ctx, ma2, mb2, ma2, g2, stream);
-    if (epilogue == CB_EPI_QUICK_GELU) return launch_gemm_2cta<CB_EPI_QUICK_GELU, false, false>(ctx, ma2, mb2, ma2, g2, stream);
-    if (epilogue == CB_EPI_GELU_TANH) return launch_gemm_2cta<CB_EPI_GELU_TANH, false, false>(ctx, ma2, mb2, ma2, g2, stream);
-    if (epilogue == CB_EPI_NONE) return launch_gemm_2cta<CB_EPI_NONE, false, false>(ctx, ma2, mb2, ma2, g2, stream);
-    return fail(ctx, CB_ERR_ARG, "gemm: unknown epilogue %d", epilogue);
-  }
   CUtensorMap ma, mb;
   uint64_t da[2] = {(uint64_t)K, (uint64_t)M}, db[2] = {(uint64_t)K, (uint64_t)N}, st[1] = {(uint64_t)K * 2};
   uint32_t ba[2] = {BK, BM}, bb[2] = {BK, (uint32_t)BN};
@@ -515,18 +208,7 @@ int gemm_f16(cb_ctx* ctx, const void* A, const void* W, const float* bias, const
   rc = make_tensor_map(ctx, &mb, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, W, db, st, bb, CU_TENSOR_MAP_SWIZZLE_128B);
   if (rc) return rc;
   GemmArgs g{bias, residual, out_f32, (__half*)out_f16, M, N, K};
-#define CB_GEMM_DISPATCH(BN_)                                                                          \
-  if (out_f32) return launch_gemm<BN_, CB_EPI_NONE, true>(ctx, ma, mb, g, stream);                      \
-  if (epilogue == CB_EPI_QUICK_GELU) return launch_gemm<BN_, CB_EPI_QUICK_GELU, false>(ctx, ma, mb, g, stream); \
-  if (epilogue == CB_EPI_GELU_TANH) return launch_gemm<BN_, CB_EPI_GELU_TANH, false>(ctx, ma, mb, g, stream);   \
-  if (epilogue == CB_EPI_NONE) return launch_gemm<BN_, CB_EPI_NONE, false>(ctx, ma, mb, g, stream);
-  if (BN == 256) {
-    CB_GEMM_DISPATCH(256)
-  } else {
-    CB_GEMM_DISPATCH(128)
-  }
-#undef CB_GEMM_DISPATCH
-  return fail(ctx, CB_ERR_ARG, "gemm: unknown epilogue %d", epilogue);
+  return BN == 256 ? dispatch_gemm<256>(ctx, ma, mb, g, epilogue, stream) : dispatch_gemm<128>(ctx, ma, mb, g, epilogue, stream);
 }
 
 }  // namespace cb

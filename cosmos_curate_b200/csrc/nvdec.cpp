@@ -408,6 +408,27 @@ int cb_mp4_cut(cb_ctx* ctx, const uint8_t* data, size_t size, int first_sample, 
   return CB_OK;
 }
 
+int cb_nvdec_probe(cb_ctx* ctx) {
+  if (!ctx) return CB_ERR_ARG;
+  CuvidApi* api = load_cuvid();
+  if (!api->error.empty()) return cb::fail(ctx, CB_ERR_NVDEC, "%s", api->error.c_str());
+  struct {  // CUVIDDECODECAPS (cuviddec.h)
+    int codec, chroma;
+    unsigned bit_depth_minus8, reserved1[3];
+    unsigned char supported, n_nvdecs;
+    unsigned short format_mask;
+    unsigned max_w, max_h, max_mb;
+    unsigned short min_w, min_h;
+    unsigned reserved2[11];
+  } caps = {};
+  caps.codec = 4, caps.chroma = 1;  // cudaVideoCodec_H264, 4:2:0, 8 bit
+  auto get_caps = (int (*)(void*))dlsym(api->handle, "cuvidGetDecoderCaps");
+  if (!get_caps) return cb::fail(ctx, CB_ERR_NVDEC, "cuvidGetDecoderCaps not found in libnvcuvid");
+  CB_CUDA(ctx, cudaSetDevice(ctx->device));
+  CB_CUDA(ctx, cudaFree(nullptr));  // a current context on this thread
+  return get_caps(&caps) == 0 && caps.supported ? 1 : 0;
+}
+
 int cb_decoder_create(cb_ctx* ctx, cb_decoder** out) {
   if (!ctx) return CB_ERR_ARG;
   if (!out) return cb::fail(ctx, CB_ERR_ARG, "decoder_create: null argument");

@@ -1,4 +1,4 @@
-// Fused frame preprocess kernels (sm_100a).
+// Fused frame preprocess kernels (sm_90a).
 //
 //  clip_preprocess_kernel : NV12 (or RGB24) frame -> YUV->RGB u8 (OpenCV BT.601 fixed point) ->
 //      antialiased bicubic resize (ATen _upsample_bicubic2d_aa arithmetic, horizontal then vertical,
@@ -134,7 +134,7 @@ __global__ void __launch_bounds__(kThreads) clip_preprocess_kernel(const __grid_
   __syncthreads();
 
   // NOTE: x_lo is a multiple of 16 pixels: a TMA box whose first byte is not 16-byte aligned in global memory
-  // faults with "illegal instruction" (measured on B200; u8 elements make this easy to hit).
+  // faults with "illegal instruction" (u8 elements make this easy to hit).
 #define CB_ISSUE_STRIP(S_)                                                                                        \
   do {                                                                                                            \
     const int s_ = (S_);                                                                                          \

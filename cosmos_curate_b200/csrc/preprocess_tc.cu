@@ -1,22 +1,22 @@
-// Third-generation fused preprocess: the horizontal antialiased-bicubic pass on the tensor pipe (tcgen05), everything else SIMT.
+// Third-generation fused preprocess: the horizontal antialiased-bicubic pass on the tensor pipe (wgmma), everything else SIMT.
 //
 // Same arithmetic contract as clip_preprocess_v2_kernel (preprocess.cu): NV12 -> RGB u8 (OpenCV or libswscale arithmetic) ->
 // torchvision Resize(res, bicubic, antialias) + CenterCrop(res) with fp32 intermediates -> round half even -> u8.  The v2
-// kernel is issue / shared-memory bound (ncu: 1.16 M shared wavefronts per 1080p frame, tensor pipe idle): 83 % of its FMAs
-// are the ~20-tap horizontal pass.  Here that pass is a banded GEMM on the tensor cores:
+// kernel is issue / shared-memory bound: 83 % of its FMAs are the ~20-tap horizontal pass.  Here that pass is a banded GEMM on the tensor cores:
 //
 //   D[(row, colour plane), x] = sum_k  A[(row, colour plane), k] * (Wh[x, k] + Wl[x, k])
 //
 //   * A = the colour-converted pixels as fp16 (0..255 is exact in fp16), written by the SIMT threads straight into the
-//     128-byte-swizzled K-major UMMA layout.  The M dimension stacks 40 source rows x 3 colour planes = 120 of the 128 UMMA
-//     rows, so one 128-row operand tile holds a whole unit of work and all three planes share the B operand (the weights).
+//     128-byte-swizzled K-major operand layout.  The M dimension stacks 40 source rows x 3 colour planes = 120 of the 128 rows of
+//     two warpgroups' m64 tiles, so one 128-row operand tile holds a whole unit of work and all three planes share the B operand
+//     (the weights).
 //   * B = the fp32 tap weights split into two fp16 terms (hi + lo, 22 significant bits: products with u8 pixels are exact in
 //     the fp32 accumulator, only the summation order differs from ATen's - the <= 1 LSB on <= 1e-4 of the pixels budget the
 //     fp32 paths already share).  An N-tile is 16 output columns; its K window is the ~100 source columns those columns
 //     tap (7 k-steps of 16), so the band is ~70 % dense instead of a dense 1080-wide GEMM.  The hi and lo terms of a tile sit
-//     side by side in the B tile (N = 32): a UMMA with M = 128 streams its A rows from shared memory in ~128 cycles whatever N
-//     is, so the number of instructions, not their width, is what costs (14 per unit).
-//   * accumulators in TMEM (64 columns per CTA: N-tile x weight term), read back with tcgen05.ld, hi + lo added, into a 64-row
+//     side by side in the B tile (N = 32): an MMA streams its A rows from shared memory whatever N is, so the number of
+//     instructions, not their width, is what costs (14 per unit and warpgroup).
+//   * accumulators in registers (2 N-tiles x 16 per thread), hi + lo added, into a 64-row
 //     ring of filtered rows in shared memory; the vertical pass (17 % of the FMAs) stays on the FMA pipe in ATen's order (it
 //     runs while the next unit's MMAs are in flight), then round / clamp / store u8.
 //
@@ -36,7 +36,7 @@
 
 namespace cb {
 
-constexpr int kNC = 32;          // output columns per CTA = two UMMA N-tiles of 16
+constexpr int kNC = 32;          // output columns per CTA = two N-tiles of 16
 constexpr int kRingRows = 64;    // ring of horizontally filtered rows
 constexpr int kRingStride = 3 * kNC + 4;  // floats per ring row: +16 B so that the epilogue's row-per-lane 16-byte stores spread over the banks
 constexpr int kMaxUnits = 128;            // units per frame column (4K: 55)
@@ -50,22 +50,13 @@ struct TcArgs {
   const int* x_lo;         // [n_slabs] first source column of the slab window (multiple of 16)
   const int* tile_k0;      // [n_slabs * 2] first k-step (16 source columns) of the N-tile inside the window
   const int* tile_nk;      // [n_slabs * 2] k-steps of the N-tile (0 = tile beyond the image)
-  const uint8_t* wtiles;   // [n_slabs][2 tiles][kb / 64][32 rows (hi | lo)][128 B] fp16, already in the swizzled UMMA layout
+  const uint8_t* wtiles;   // [n_slabs][2 tiles][kb / 64][32 rows (hi | lo)][128 B] fp16, already in the swizzled operand layout
   const int *ymin, *ysize;
   const int* unit_last;    // [n_units] output rows complete once unit u has been filtered
   const float* wy;
   int ty;
   uint8_t* out;  // [n][3][res][res]
 };
-
-__device__ __forceinline__ void tmem_ld_32x32b_x16(uint32_t taddr, uint32_t* r) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]), "=r"(r[10]),
-        "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr)
-      : "memory");
-}
 
 // two integers 0..255 -> packed fp16 pair, exactly: 0x6400 | v is the fp16 1024 + v, and (1024 + v) - 1024 is exact
 __device__ __forceinline__ uint32_t pack_u8_pair_f16(int a, int b) {
@@ -92,23 +83,17 @@ __global__ void __launch_bounds__(kTcThreads, 2)
   int* sUL = sY + 2 * kVRows;                                 // [kMaxUnits] copy of unit_last (a global load per phase would sit on the critical path)
   uint64_t* bars = reinterpret_cast<uint64_t*>(sUL + kMaxUnits);
   uint64_t* raw_full = bars;
-  uint64_t* mma_done = bars + 1;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 2);
 
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const int tid = threadIdx.x, warp = __shfl_sync(0xffffffffu, tid >> 5, 0), lane = tid & 31;  // warp index: provably warp-uniform
   const int slab = blockIdx.x, frame = blockIdx.y;
   const int slot = a.slots[frame];
   const int x_lo = a.x_lo[slab], x0 = slab * a.nc;
   const int ncols = min(a.nc, a.res - x0);
 
   if (tid == 0) {
-    mbar_init(raw_full, 1), mbar_init(mma_done, 1);
+    mbar_init(raw_full, 1);
     fence_barrier_init();
     tma_prefetch_desc(&map_y), tma_prefetch_desc(&map_uv);
-  }
-  if (warp == 1) {
-    tmem_alloc(tmem_slot, 64);
-    tmem_relinquish();
   }
   {
     const uint4* src = reinterpret_cast<const uint4*>(a.wtiles + (size_t)slab * 2 * b_tile);
@@ -116,10 +101,7 @@ __global__ void __launch_bounds__(kTcThreads, 2)
     for (int i = tid; i < (2 * b_tile) >> 4; i += kTcThreads) dst[i] = src[i];
     for (int i = tid; i < a.n_units; i += kTcThreads) sUL[i] = a.unit_last[i];
   }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = *tmem_slot;
   const uint32_t raw_tx = (uint32_t)((ru + ru / 2) * kw);
   auto issue = [&](int u) {
     const int ys = a.y_begin + u * ru;
@@ -129,11 +111,12 @@ __global__ void __launch_bounds__(kTcThreads, 2)
   };
   if (tid == 0) issue(0);
 
-  constexpr uint32_t idesc = umma_idesc_f16(128, 32, 0);  // N = 32: the hi and lo weight terms of 16 output columns side by side
-  // per-CTA constants of the MMA issuer: k-step windows of the two N-tiles and the operand descriptor bases (16-byte units)
+  // per-CTA constants of the MMA issue: k-step windows of the two N-tiles and the operand descriptor bases (16-byte units)
   const int nk0 = a.tile_nk[slab * 2], nk1 = a.tile_nk[slab * 2 + 1], k00 = a.tile_k0[slab * 2], k01 = a.tile_k0[slab * 2 + 1];
   const int nkm = nk0 > nk1 ? nk0 : nk1;
-  const uint64_t desc_a0 = umma_desc_sw128(smem_u32(sA)), desc_b0 = umma_desc_sw128(smem_u32(sB));
+  // warps 0-7 are the two warpgroups that issue the MMAs: warpgroup w owns operand rows 64w..64w+63
+  const uint64_t desc_a0 = wgmma_desc_sw128(smem_u32(sA) + (uint32_t)((warp >> 2) & 1) * (64 * 128)), desc_b0 = wgmma_desc_sw128(smem_u32(sB));
+  float acc[2][16];  // [N-tile][hi-weight partial sums of columns 0..15 | lo-weight partial sums]
   const uint32_t b_tile16 = (uint32_t)b_tile >> 4;
   const int q4 = kw >> 2;
   const int rp0 = tid / q4, xg0 = tid - rp0 * q4, drp = kTcThreads / q4, dxg = kTcThreads - drp * q4;  // item walk of the convert phase
@@ -152,7 +135,7 @@ __global__ void __launch_bounds__(kTcThreads, 2)
     }
   };
   // vertical pass for the output rows completed by unit `uv` (ATen order: first product, then FMAs), round half even.  It runs while
-  // the NEXT unit's MMAs are in flight (their issue-to-commit latency, ~2 k cycles of dependent accumulation, used to be a sleep).
+  // the NEXT unit's MMAs are in flight.
   auto vertical = [&](int uv) {
     const int u = uv;
     (void)u;
@@ -255,57 +238,50 @@ __global__ void __launch_bounds__(kTcThreads, 2)
     }
     fence_proxy_async();  // generic-proxy writes of the operand -> visible to the tensor core (async proxy)
     __syncthreads();
-    if (tid == 0) {
-      if (u + 1 < a.n_units) issue(u + 1);  // the raw window is free again
-      tc_fence_after();
-      // Four independent accumulators - (N-tile, weight term) - interleaved k-step by k-step: a chain of accumulations into ONE
-      // TMEM tile serialises on the MMA pipeline latency (measured: 28 back-to-back dependent MMAs cost ~3.5 k cycles, 44 % of the
-      // warp samples slept on the commit barrier); hi and lo partial sums are added in the epilogue instead.
-      // One MMA per (N-tile, k-step): a UMMA with M = 128 streams its 128 A rows from shared memory in ~128 cycles whatever N is
-      // (measured: 28 N=16 MMAs per unit cost ~3.5 k cycles, 44 % of the warp samples slept on the commit), so the hi and lo weight
-      // terms ride in the SAME instruction as N = 32 - two accumulators per tile (TMEM columns 0..15 | 16..31), added in the epilogue.
+    if (tid == 0 && u + 1 < a.n_units) issue(u + 1);  // the raw window is free again
+    if (warp < 8) {
+      // One MMA per (N-tile, k-step), N = 32: the hi and lo weight terms of 16 output columns ride in the same instruction as two
+      // accumulator column groups (added in the epilogue), and the two N-tiles are independent accumulation chains.
+      wgmma_fence();
       for (int kk = 0; kk < nkm; ++kk) {
         const uint64_t kb_off = (uint64_t)(((kk >> 2) << 8) + ((kk & 3) << 1));  // chunk of 64 k: 32 rows x 128 B = 4096 B, k-step: 32 B
 #pragma unroll
         for (int j = 0; j < 2; ++j) {
-          if (kk >= (j ? nk1 : nk0)) continue;
-          const int qa = (j ? k01 : k00) + kk;
+          // no branch inside the MMA sequence: past its own last k-step the shorter tile multiplies zero weights (the weight tiles are
+          // zero-padded to kb) with the last operand columns of the window
+          const int qa = min((j ? k01 : k00) + kk, (kw >> 4) - 1);
           const uint64_t da = desc_a0 + (uint64_t)(((qa >> 2) << 10) + ((qa & 3) << 1));  // chunk: 16384 B
-          umma_f16(tmem + (uint32_t)(j * 32), da, desc_b0 + (uint64_t)(j * b_tile16) + kb_off, idesc, kk != 0);
+          wgmma_m64n32k16(acc[j], da, desc_b0 + (uint64_t)(j * b_tile16) + kb_off, kk != 0);
         }
       }
-      umma_commit(mma_done);
+      wgmma_commit();
     }
     if (u > 0) vertical(u - 1);
     __syncthreads();  // the epilogue below overwrites ring rows the vertical pass was still reading
-    if (a.wait_ns) mbar_wait_parked(mma_done, u & 1, a.wait_ns);  // suspend-time hint: do not burn the co-resident CTA's issue slots
-    else mbar_wait(mma_done, u & 1);
-    tc_fence_after();
-    // ---- epilogue: the filtered rows of this unit -> ring (warp = lane quarter x N-tile)
+    // ---- epilogue: the filtered rows of this unit -> ring.  Lane l of warp w holds rows 16w + l/4 (+ 8), columns 2(l%4) + {0, 1} of
+    // every 8-column block: blocks 0-1 = hi-weight sums of output columns 0..15, blocks 2-3 = lo-weight sums of the same columns.
     if (warp < 8) {
-      const int lq = warp & 3, half = warp >> 2;
-      uint32_t v[16], vl[16];
-      tmem_ld_32x32b_x16(tmem + ((uint32_t)(lq * 32) << 16) + (uint32_t)(half * 32), v);        // hi-weight partial sums
-      tmem_ld_32x32b_x16(tmem + ((uint32_t)(lq * 32) << 16) + (uint32_t)(half * 32 + 16), vl);  // lo-weight partial sums
-      tmem_ld_wait();
-      const int l = lq * 32 + lane;
-      if (l < 3 * ru) {
-        const int ch = l / ru, r = l - ch * ru;
-        float4* dst = reinterpret_cast<float4*>(ring + ((u * ru + r) & (kRingRows - 1)) * kRingStride + ch * kNC + half * 16);
+      wgmma_wait<0>();
 #pragma unroll
-        for (int q = 0; q < 4; ++q)
-          dst[q] = make_float4(__uint_as_float(v[4 * q]) + __uint_as_float(vl[4 * q]), __uint_as_float(v[4 * q + 1]) + __uint_as_float(vl[4 * q + 1]),
-                               __uint_as_float(v[4 * q + 2]) + __uint_as_float(vl[4 * q + 2]), __uint_as_float(v[4 * q + 3]) + __uint_as_float(vl[4 * q + 3]));
+      for (int h = 0; h < 2; ++h) {
+        const int l = warp * 16 + (lane >> 2) + 8 * h;
+        if (l >= 3 * ru) continue;
+        const int ch = l / ru, r = l - ch * ru;
+        float* dst = ring + ((u * ru + r) & (kRingRows - 1)) * kRingStride + ch * kNC + 2 * (lane & 3);
+#pragma unroll
+        for (int j = 0; j < 2; ++j) {
+#pragma unroll
+          for (int b = 0; b < 2; ++b)
+            *reinterpret_cast<float2*>(dst + j * 16 + b * 8) =
+                make_float2(acc[j][4 * b + 2 * h] + acc[j][8 + 4 * b + 2 * h], acc[j][4 * b + 2 * h + 1] + acc[j][8 + 4 * b + 2 * h + 1]);
+        }
       }
     }
-    tc_fence_before();
     __syncthreads();
   }
   stage_taps(a.n_units - 1);
   __syncthreads();
   vertical(a.n_units - 1);
-  __syncthreads();
-  if (warp == 1) tmem_dealloc(tmem, 64);
 }
 
 // u8 [n][3][res][res] -> normalised output: typed NCHW (mode 1) or zero-padded patch rows [n][(res/p)^2][k_pad] (mode 2)

@@ -1,9 +1,9 @@
-// Non-GEMM kernels of the image tower (sm_100a): LayerNorm, token assembly, attention, pooled tail.
+// Non-GEMM kernels of the image tower (sm_90a): LayerNorm, token assembly, attention, pooled tail.
 //   layernorm_kernel       fp32 residual stream -> fp16 normalised activations (HBM-bound: 6 B/element)
 //   assemble_kernel        patch-embed output + [CLS] + position embedding (+ CLIP pre_layrnorm) -> residual stream
 //   attention_kernel       softmax(Q K^T / sqrt(d)) V per (image, head); K/V resident in shared memory,
 //                          mma.sync m16n8k16 with fp32 online softmax (4 % of the tower's FLOPs; the dense
-//                          Linear layers are the tcgen05 kernel in gemm.cu)
+//                          Linear layers are the wgmma kernel in gemm.cu)
 //   clip_tail_kernel       post_layernorm(CLS) -> visual_projection -> L2 normalise -> aesthetic affine head
 #include <cuda_fp16.h>
 
@@ -558,17 +558,14 @@ int assemble_tokens(cb_ctx* ctx, const float* patch, const float* cls, const flo
   return CB_OK;
 }
 
-int attention_tc(cb_ctx* ctx, const void* qkv, void* out, int n, int tokens, int heads, int head_dim, cudaStream_t stream, bool* launched);
-int attention_tc2(cb_ctx* ctx, const void* qkv, void* out, int n, int tokens, int heads, int head_dim, cudaStream_t stream, bool* launched);
+int attention_wgmma(cb_ctx* ctx, const void* qkv, void* out, int n, int tokens, int heads, int head_dim, cudaStream_t stream, bool* launched);
 
 int attention_f16(cb_ctx* ctx, const void* qkv, void* out, int n, int tokens, int heads, int head_dim, cudaStream_t stream) {
   if (!qkv || !out) return fail(ctx, CB_ERR_ARG, "attention: null operand");
   if (n <= 0) return CB_OK;
-  {  // head_dim 64, 129..257 tokens (ViT-L/14): tcgen05 kernel (attention_tc.cu); everything else: mma.sync kernel below
+  {  // head_dim 64, 129..257 tokens (ViT-L/14): wgmma kernel (attention_wgmma.cu); everything else: mma.sync kernel below
     bool launched = false;
-    int rc = attention_tc2(ctx, qkv, out, n, tokens, heads, head_dim, stream, &launched);  // two threads per row (CB_ATTN_KERNEL=tc1|mma skips it)
-    if (rc || launched) return rc;
-    rc = attention_tc(ctx, qkv, out, n, tokens, heads, head_dim, stream, &launched);  // one thread per row
+    const int rc = attention_wgmma(ctx, qkv, out, n, tokens, heads, head_dim, stream, &launched);  // CB_ATTN_KERNEL=mma skips it
     if (rc || launched) return rc;
   }
   if (tokens <= 0 || heads <= 0 || head_dim % 8 || head_dim > 80 || head_dim < 16)

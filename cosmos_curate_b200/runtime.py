@@ -6,6 +6,7 @@ Nothing here computes on the data path; every operation is a call into libcurate
 from __future__ import annotations
 
 import ctypes as C
+import os
 import weakref
 
 import numpy as np
@@ -13,6 +14,13 @@ import torch
 
 from . import _lib
 from ._lib import SurfacePool, VitCfg, check
+
+try:
+    from loguru import logger
+except ImportError:
+    import logging
+
+    logger = logging.getLogger(__name__)
 
 CLIP_MEAN = (0.48145466, 0.4578275, 0.40821073)  # reference: cosmos_curate/models/clip.py:57-60
 CLIP_STD = (0.26862954, 0.26130258, 0.27577711)
@@ -352,11 +360,36 @@ def mp4_index(data, ctx: Context | None = None) -> dict:
             "pts": pts, "sync": sync}  # fmt: skip
 
 
+_NVDEC_OK: dict[int, bool] = {}
+
+
+def nvdec_available(ctx: Context) -> bool:
+    """cb_nvdec_probe, once per device: False where libnvcuvid loads but the driver reports no H.264 decode for this process
+    (containers granted only the compute capability).  Decode requests then take the host path (host_decode.py: same pictures,
+    same surface pools) after one warning; CURATE_B200_DECODE=nvdec makes that an error instead.  A missing libnvcuvid raises."""
+    if ctx.device not in _NVDEC_OK:
+        rc = ctx.lib.cb_nvdec_probe(ctx.h)
+        if rc < 0:
+            check(rc, "cb_nvdec_probe", ctx.h)
+        if rc == 0:
+            if os.environ.get("CURATE_B200_DECODE") == "nvdec":
+                raise _lib.CurateB200Error(-4, "cb_nvdec_probe", "the driver reports no H.264 decode for this device and CURATE_B200_DECODE=nvdec")
+            logger.warning(f"NVDEC of cuda:{ctx.device} is not usable from this process (cuvidGetDecoderCaps: no H.264 support): "
+                           "clips are decoded on the HOST with libavcodec - far below the hardware decode rate")  # fmt: skip
+        _NVDEC_OK[ctx.device] = rc == 1
+    return _NVDEC_OK[ctx.device]
+
+
 class Decoder:
-    """One NVDEC session (cb_decoder_*).  Not thread-safe: use one per host thread."""
+    """One decode session: NVDEC (cb_decoder_*), or libavcodec on the host where the device's NVDEC is not usable (nvdec_available).
+    Not thread-safe: use one per host thread."""
 
     def __init__(self, ctx: Context):
         self.ctx, self.lib = ctx, ctx.lib
+        self.host = not nvdec_available(ctx)
+        if self.host:
+            self.h = True
+            return
         h = C.c_void_p()
         check(self.lib.cb_decoder_create(ctx.h, C.byref(h)), "cb_decoder_create", ctx.h)
         self.h = h
@@ -364,8 +397,55 @@ class Decoder:
 
     def close(self):
         if getattr(self, "h", None):
-            self.lib.cb_decoder_destroy(self.h)
+            if not self.host:
+                self.lib.cb_decoder_destroy(self.h)
             self.h = None
+
+    def _host_decode(self, buf, ids, pool, slots, seek_keyframes: bool) -> dict:
+        """decode() on the host: the same request checks and statistics as cb_decoder_decode_ex, pictures uploaded as NV12."""
+        from . import host_decode
+
+        idx = mp4_index(buf, self.ctx)  # CB_ERR_DEMUX on anything that is not an mp4 with a video track
+        n = idx["n_samples"]
+        w2, h2 = (idx["width"] + 1) & ~1, (idx["height"] + 1) & ~1
+        st = {"frames_decoded": 0, "frames_emitted": 0, "coded": ((idx["width"] + 15) & ~15, (idx["height"] + 15) & ~15), "size": (idx["width"], idx["height"])}
+        if pool is not None and len(ids) == 0:
+            return st
+        if pool is not None:
+            if np.any(np.diff(ids) < 0) or ids[0] < 0:
+                raise _lib.CurateB200Error(-2, "cb_decoder_decode", "frame ids must be ascending")
+            if ids[-1] >= n:
+                raise _lib.CurateB200Error(-2, "cb_decoder_decode", f"frame id {ids[-1]} beyond the clip ({n} frames)")
+            if (pool.desc.width, pool.desc.height) != (w2, h2):
+                raise _lib.CurateB200Error(-4, "cb_decoder_decode", f"decode: pool is {pool.desc.width}x{pool.desc.height}, the stream {w2}x{h2}")
+            if slots.min() < 0 or slots.max() >= pool.buf.shape[0]:
+                raise _lib.CurateB200Error(-2, "cb_decoder_decode", "destination slot out of range")
+        last = int(ids[-1]) if pool is not None else n - 1
+        runs = [(0, last)]
+        if seek_keyframes and pool is not None and not idx["has_ctts"]:  # no reordering: display index = sample index
+            starts = np.flatnonzero(idx["sync"])
+            gop = np.searchsorted(starts, ids, side="right") - 1
+            runs = [(int(starts[g]), int(ids[gop == g].max())) for g in np.unique(gop)]
+        where: dict[int, list[int]] = {}
+        if pool is not None:
+            for i, s in zip(ids.tolist(), slots.tolist()):
+                where.setdefault(i, []).append(s)
+        emitted = 0
+
+        def on_frame(i, y, u, v):
+            nonlocal emitted
+            if i in where:
+                _upload_yuv420(pool, where[i], y, u, v)
+                emitted += len(where[i])
+
+        try:
+            st["frames_decoded"], _, _ = host_decode.decode(buf, idx["sync"], runs, on_frame)
+        except ValueError as exc:
+            raise _lib.CurateB200Error(-4, "cb_decoder_decode", f"decode: {exc}") from exc
+        if pool is not None and emitted != len(ids):
+            raise _lib.CurateB200Error(-4, "cb_decoder_decode", f"decode: {emitted} of {len(ids)} frames delivered")
+        st["frames_emitted"] = emitted
+        return st
 
     def __del__(self):
         try:
@@ -381,6 +461,8 @@ class Decoder:
         ids = np.ascontiguousarray(frame_ids, dtype=np.int32)
         slots = np.ascontiguousarray(dst_slots, dtype=np.int32)
         assert len(ids) == len(slots)
+        if self.host:
+            return self._host_decode(buf, ids, pool, slots, seek_keyframes)
         st = _lib.DecodeStats()
         flags = _lib.DECODE_SEEK_SYNC if seek_keyframes else 0
         check(self.lib.cb_decoder_decode_ex(self.h, buf.ctypes.data, buf.size, ids.ctypes.data_as(C.POINTER(C.c_int32)), len(ids),
@@ -390,9 +472,24 @@ class Decoder:
                 "size": (st.width, st.height)}  # fmt: skip
 
 
+def _upload_yuv420(pool: Pool, slots, y: np.ndarray, u: np.ndarray, v: np.ndarray) -> None:
+    """One decoded 4:2:0 picture as NV12 into `slots` of the pool (the layout NVDEC's mapped surfaces are copied into)."""
+    rows, pitch = pool.buf.shape[1:]
+    luma_rows = pool.desc.luma_rows
+    nv12 = np.zeros((rows, pitch), dtype=np.uint8)
+    nv12[: y.shape[0], : y.shape[1]] = y
+    nv12[luma_rows : luma_rows + u.shape[0], 0 : 2 * u.shape[1] : 2] = u
+    nv12[luma_rows : luma_rows + v.shape[0], 1 : 2 * v.shape[1] : 2] = v
+    t = torch.from_numpy(nv12).to(pool.buf.device)
+    for s in slots:
+        pool.buf[s].copy_(t)
+
+
 def decode_discard(dec: Decoder, data) -> int:
     """Decode every picture of the clip and deliver none; returns the number decoded (NVDEC ceiling measurement)."""
     buf = _as_u8(data)
+    if dec.host:
+        return dec._host_decode(buf, None, None, None, False)["frames_decoded"]
     st = _lib.DecodeStats()
     check(dec.lib.cb_decoder_decode_ex(dec.h, buf.ctypes.data, buf.size, None, 0, None, None, _lib.DECODE_DISCARD_ALL, C.byref(st)),
           "cb_decoder_decode_ex", dec.ctx.h)
@@ -402,6 +499,23 @@ def decode_discard(dec: Decoder, data) -> int:
 def decode_thumbnails(dec: Decoder, data, out_w: int, out_h: int, n_frames: int) -> torch.Tensor:
     """Every frame of the clip as uint8 cuda [n, out_h, out_w, 3] (cb_decoder_decode_thumbnails)."""
     buf = _as_u8(data)
+    if dec.host:  # one decode pass; a batch of frames at a time through a surface pool and the same bilinear kernel
+        from . import host_decode
+
+        idx = mp4_index(buf, dec.ctx)
+        n, batch, parts = min(n_frames, idx["n_samples"]), 64, []
+        pool = alloc_nv12_pool(dec.ctx, batch, idx["width"], idx["height"])
+
+        def on_frame(i, y, u, v):
+            _upload_yuv420(pool, [i % batch], y, u, v)
+            if i % batch == batch - 1 or i == n - 1:
+                parts.append(dec.ctx.preprocess_bilinear_u8(pool, out_w, out_h, slots=np.arange(i % batch + 1, dtype=np.int32)))
+
+        try:
+            host_decode.decode(buf, idx["sync"], [(0, n - 1)], on_frame)
+        except ValueError as exc:
+            raise _lib.CurateB200Error(-4, "cb_decoder_decode_thumbnails", f"decode: {exc}") from exc
+        return torch.cat(parts) if parts else torch.empty((0, out_h, out_w, 3), dtype=torch.uint8, device=f"cuda:{dec.ctx.device}")
     out = torch.empty((n_frames, out_h, out_w, 3), dtype=torch.uint8, device=f"cuda:{dec.ctx.device}")
     st = _lib.DecodeStats()
     check(dec.lib.cb_decoder_decode_thumbnails(dec.h, buf.ctypes.data, buf.size, out_w, out_h, out.data_ptr(), n_frames, C.byref(st)),

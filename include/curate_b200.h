@@ -37,7 +37,7 @@ typedef struct cb_vit cb_vit;
 
 /* ---- context ------------------------------------------------------------------------------------ */
 int cb_abi_version(void);
-/* Creates a context on CUDA device `device` (must be sm_100).  Replaces the implicit torch/CV-CUDA
+/* Creates a context on CUDA device `device` (must be sm_90).  Replaces the implicit torch/CV-CUDA
  * device setup of nvcodec_utils.py:337 (device_id hard-coded to 0 there) and clip.py:39. */
 int cb_init(int device, cb_ctx** out);
 void cb_destroy(cb_ctx* ctx);
@@ -206,6 +206,10 @@ int cb_mp4_index(cb_ctx* ctx, const uint8_t* data, size_t size, cb_mp4_info* inf
 int cb_mp4_cut(cb_ctx* ctx, const uint8_t* data, size_t size, int first_sample, int n_samples, uint8_t* out, size_t out_cap,
                size_t* out_size);
 
+/* 1 when the device decodes 8-bit 4:2:0 H.264 for this process (cuvidGetDecoderCaps through the libnvcuvid the decoder itself
+ * loads), 0 when the driver reports no support (e.g. a container granted only the compute capability), < 0 on error
+ * (libnvcuvid missing). */
+int cb_nvdec_probe(cb_ctx* ctx);
 /* One NVDEC session (parser + decoder + copy stream); use one per host thread, reuse it across clips. */
 int cb_decoder_create(cb_ctx* ctx, cb_decoder** out);
 void cb_decoder_destroy(cb_decoder* dec);

@@ -29,9 +29,10 @@ def test_shot_flops_per_window_matches_the_architecture():
     assert abs(bench.shot_flops_per_window(50) * 2 - total) / total < 1e-6  # linear in the frame count
 
 
-def test_ncu_traffic_reads_the_committed_capture():
-    t = bench.ncu_traffic()
-    assert t["_source"].startswith("profiles/") and t["gemm_tcgen05_2cta"] > 1e8 and t["layernorm_kernel"] > 1e8
+def test_steps_and_dump_outputs_arguments():
+    r = subprocess.run([sys.executable, str(ROOT / "bench.py"), "--steps", "0", "--dump-outputs", "x"], capture_output=True, text=True, cwd=str(ROOT))
+    assert r.returncode == 2 and "--steps must be at least 1" in r.stderr
+    assert "--dump-outputs DIR" in subprocess.run([sys.executable, str(ROOT / "bench.py"), "--help"], capture_output=True, text=True, cwd=str(ROOT)).stdout
 
 
 def test_reference_arm_prints_one_contract_line():

@@ -1,4 +1,4 @@
-"""GPU parity tests (B200): every call goes through the C ABI of libcurate_b200.so.
+"""GPU parity tests (H100): every call goes through the C ABI of libcurate_b200.so.
 
 Integer / byte stages are compared bit-exactly with the oracle where the arithmetic is pinned
 (colour conversion, frame indices), within the stated fp32-summation budget where it is not
@@ -81,34 +81,29 @@ def test_attention(ctx, n, t, heads, hd):
 
 
 
-def test_attention_tcgen05_and_mma_kernels_agree(ctx, monkeypatch):
-    """head_dim 64 / 129..257 tokens runs on tcgen05 (attention_tc.cu); CB_ATTN_KERNEL=mma forces the mma.sync kernel."""
+def test_attention_wgmma_and_mma_kernels_agree(ctx, monkeypatch):
+    """head_dim 64 / 129..257 tokens runs on wgmma (attention_wgmma.cu); CB_ATTN_KERNEL=mma forces the mma.sync kernel."""
     g = torch.Generator(device="cuda").manual_seed(11)
     qkv = (torch.randn(20, 257, 3 * 1024, device="cuda", generator=g) * 2.0).half()
     qkv[:, :, 5] += 6.0  # a dominant query/key channel: sharp softmax rows
     tc = ctx.attention(qkv, 16).float()
-    monkeypatch.setenv("CB_ATTN_KERNEL", "tc1")  # first-generation tcgen05 kernel (one thread per row)
-    tc1 = ctx.attention(qkv, 16).float()
-    torch.testing.assert_close(tc, tc1, rtol=2e-3, atol=1e-3)
     monkeypatch.setenv("CB_ATTN_KERNEL", "mma")
     mma = ctx.attention(qkv, 16).float()
     torch.testing.assert_close(tc, mma, rtol=1e-2, atol=4e-3)
     again = ctx.attention(qkv, 16).float()
     assert torch.equal(mma, again)
     monkeypatch.delenv("CB_ATTN_KERNEL")
-    # The second-generation kernel issues a tile's four P.V chunk products in the fixed order 0, 2, 1, 3: repeat runs are bitwise equal
-    # (also under load: 300 units per CTA-wave with different arrival timing of the two half-row streams).
+    # every product of the wgmma kernel is issued in a fixed order by the warpgroup that owns the rows: repeat runs are bitwise equal
     for _ in range(3):
         assert torch.equal(tc, ctx.attention(qkv, 16).float())
 
 
-@pytest.mark.parametrize("kernel", ["1cta", "2cta"])
-@pytest.mark.parametrize(("m", "n", "k"), [(300, 256, 192), (257, 136, 72), (1000, 1024, 1024), (5000, 768, 640), (4096, 4304, 1152)])
-def test_gemm_both_kernels_with_tails(ctx, monkeypatch, kernel, m, n, k):
-    """Force the 1-CTA and the 2-CTA (cta_group::2) kernels through M/N/K tails and the activation epilogue."""
+@pytest.mark.parametrize(("m", "n", "k"), [(300, 256, 192), (257, 136, 72), (1000, 1024, 1024), (5000, 768, 640), (4096, 4304, 1152),
+                                             (129, 264, 136), (20000, 512, 200), (64, 72, 72), (2570, 1000, 264), (33000, 1280, 320)])
+def test_gemm_with_tails(ctx, m, n, k):
+    """Both tile widths through M/N/K tails, the activation epilogue and the residual epilogue."""
     from cosmos_curate_b200 import _lib
 
-    monkeypatch.setenv("CB_GEMM_KERNEL", kernel)
     g = torch.Generator(device="cuda").manual_seed(m * 7 + n)
     a = (torch.randn(m, k, device="cuda", generator=g) * 0.5).half()
     w = (torch.randn(n, k, device="cuda", generator=g) * 0.5).half()

@@ -5,7 +5,7 @@
   on CLIP ViT-L/14.  Round 1 converted with OpenCV / CV-CUDA semantics and claimed the difference to swscale was "absorbed by the
   1e-3 tolerance"; measured here it is NOT (1.2e-2 on the dark title frames), so the fused kernel now has libswscale's own
   arithmetic (CB_FMT_NV12_SWS) and the stages default to it: the RGB is byte-identical, the embeddings within 1e-3.
-* batch invariance at the bench shape: 264 frames through the 2-CTA GEMM + attention_tc2 + chunking vs the same frames at n=3.
+* batch invariance at the bench shape: 264 frames through the wgmma GEMM + attention_wgmma + chunking vs the same frames at n=3.
 * activation outliers: real CLIP-L/14 has a few residual-stream channels two orders of magnitude above the rest; seeded
   Gaussian weights do not.  A stress configuration plants such channels and checks the fp16 qkv / mlp activations survive.
 * the reference's real-weight goldens 4.8575 / 3.7989 +- 0.002 (test_aesthetic_filter.py:33-35) - skipped unless the
@@ -96,7 +96,7 @@ def test_real_input_path_embeddings_swscale_vs_nvdec_l14(ctx):
 
 
 def test_batch_invariance_at_bench_shape_l14(ctx):
-    """n=264 (2-CTA GEMM tiles, attention_tc2 over 4224 units, max_batch chunking) vs n=3: same frames, same embeddings."""
+    """n=264 (128 x 256 GEMM tiles, attention_wgmma over 4224 units, max_batch chunking) vs n=3: same frames, same embeddings."""
     from cosmos_curate_b200.runtime import VitTower
 
     cfg = vit.CLIP_VIT_L14

@@ -288,7 +288,7 @@ def test_stage_perf_covers_the_work_and_concurrent_decode_errors(ctx):
 
 
 def test_fused_stage_is_deterministic_at_l14_shape(ctx):
-    """ADVICE r1: clips near score_threshold must not flip between runs - the L/14 shape (attention_tc2) through the stage,
+    """ADVICE r1: clips near score_threshold must not flip between runs - the L/14 shape (attention_wgmma) through the stage,
     twice, bitwise equal scores and embeddings; identical clips inside one call agree too."""
     from cosmos_curate_b200.models.clip_aesthetics import CLIPAestheticScorer
     from cosmos_curate_b200.runtime import VitTower, get_context

@@ -1,113 +1,112 @@
-"""Differential tests against the reference's OWN functions, imported / executed from /root/reference, on randomly generated
-inputs (hypothesis).  They run in the build container only - the GPU box has no reference checkout - and complement the committed
-golden vectors: frame-index math (decoder_utils.find_closest_indices / sample_closest), fixed-stride spans, chunk sizes and the
-stage-replay comparator must agree with the reference on inputs nobody hand-picked."""
+"""Differential tests against the reference's OWN functions on randomly generated inputs nobody hand-picked: frame-index math
+(decoder_utils.find_closest_indices / sample_closest), fixed-stride spans, chunk sizes, shot logic, the video-tube formulation and
+the stage-replay comparator must agree with the reference.
+
+The inputs are rebuilt from seeds (oracle/reference_cases.py); what the reference's functions returned on them was stored in
+tests/golden/reference_live.json.gz by `python -m oracle.make_reference_golden`, so the comparison runs without a checkout of the
+reference."""
 
 from __future__ import annotations
 
-import numpy as np
-import pytest
-from hypothesis import HealthCheck, given, settings
-from hypothesis import strategies as st
+import gzip
+import hashlib
+import json
 
+import numpy as np
+
+from conftest import GOLDEN
 from cosmos_curate_b200 import compare as C
 from cosmos_curate_b200 import sampling as S
 from cosmos_curate_b200 import spans as SP
-from oracle import ref_import
+from oracle import reference_cases as RC
 
-pytestmark = pytest.mark.skipif(not ref_import.available(), reason="needs /root/reference (build container)")
-_cfg = settings(max_examples=150, deadline=None, suppress_health_check=[HealthCheck.too_slow])
-
-
-@st.composite
-def _timestamps(draw):
-    """Sorted float32 presentation times: constant or variable frame rate, optional dropped frames, optional start offset."""
-    n = draw(st.integers(2, 400))
-    fps = draw(st.sampled_from([10.0, 23.976, 24.0, 25.0, 29.97, 30.0, 50.0, 59.94, 60.0]))
-    t = np.arange(n, dtype=np.float64) / fps + draw(st.sampled_from([0.0, 0.0, 0.033, 1.5]))
-    if draw(st.booleans()):
-        t = t + np.cumsum(draw(st.lists(st.floats(0.0, 0.02), min_size=n, max_size=n)))  # variable frame rate
-    if draw(st.booleans()) and n > 10:
-        keep = np.ones(n, bool)
-        keep[draw(st.lists(st.integers(1, n - 2), max_size=n // 5))] = False  # dropped frames
-        t = t[keep]
-    return np.sort(t.astype(np.float32))
+WANT = json.loads(gzip.decompress((GOLDEN / "reference_live.json.gz").read_bytes()))
+SEEDS = range(RC.N_CASES)
+assert WANT["n_cases"] == RC.N_CASES
 
 
-@_cfg
-@given(ts=_timestamps(), rate=st.sampled_from([0.5, 1.0, 2.0, 3.0, 4.0, 7.5, 8.0, 16.0, 30.0, 100.0]), endpoint=st.booleans(), dedup=st.booleans())
-def test_sample_closest_agrees_with_the_reference(ts, rate, endpoint, dedup):
-    du = ref_import.decoder_utils()
-    want = du.sample_closest(ts, sample_rate=rate, start=ts[0], stop=ts[-1], endpoint=endpoint, dedup=dedup)
-    got = S.sample_closest(ts, rate, start=ts[0], stop=ts[-1], endpoint=endpoint, dedup=dedup)
-    for g, w in zip(got, want):
+def _sample_closest_agrees_with_the_reference(seed):
+    c, want = RC.sample_closest_case(seed), WANT["sample_closest"][seed]
+    ts = c["ts"]
+    got = S.sample_closest(ts, c["rate"], start=ts[0], stop=ts[-1], endpoint=c["endpoint"], dedup=c["dedup"])
+    assert len(got) == len(want["sample"])
+    for g, w in zip(got, want["sample"]):
         assert np.array_equal(np.asarray(g), np.asarray(w))
-    dst = np.linspace(float(ts[0]) - 0.3, float(ts[-1]) + 0.3, 57).astype(np.float32)
-    assert np.array_equal(S.find_closest_indices(ts, dst), du.find_closest_indices(ts, dst))
+    assert np.array_equal(S.find_closest_indices(ts, c["dst"]), np.asarray(want["closest"]))
 
 
-@_cfg
-@given(end=st.floats(0.0, 400.0), clip_len=st.floats(0.1, 60.0), stride=st.floats(0.05, 90.0), min_len=st.floats(0.0, 30.0), session=st.text(min_size=0, max_size=12))
-def test_fixed_stride_spans_and_uuids_agree_with_the_reference(end, clip_len, stride, min_len, session):
-    f = ref_import.fixed_stride_functions()
-    want = f["_make_spans_fixed_stride"](0.0, end, clip_len, stride, min_len)
-    got = SP.make_spans_fixed_stride(0.0, end, clip_len, stride, min_len)
-    assert [(float.hex(a), float.hex(b)) for a, b in got] == [(float.hex(a), float.hex(b)) for a, b in want]
-    assert SP.make_clip_uuids(session, got[:50]) == f["_make_clip_uuids"](session, want[:50])
+def _fixed_stride_spans_and_uuids_agree_with_the_reference(seed):
+    c, want = RC.fixed_stride_case(seed), WANT["fixed_stride"][seed]
+    got = SP.make_spans_fixed_stride(0.0, c["end"], c["clip_len"], c["stride"], c["min_len"])
+    assert [[float.hex(a), float.hex(b)] for a, b in got] == want["spans"]
+    assert [str(u) for u in SP.make_clip_uuids(c["session"], got[:50])] == want["uuids"]
 
 
-@_cfg
-@given(durs=st.lists(st.floats(0.0, 40.0), max_size=120), per_chunk=st.integers(1, 40))
-def test_chunk_sizes_agree_with_the_reference(durs, per_chunk):
-    spans = [(float(i), float(i) + d) for i, d in enumerate(durs)]
+def _chunk_sizes_agree_with_the_reference(seed):
+    c = RC.chunk_case(seed)
+    spans = [(float(i), float(i) + d) for i, d in enumerate(c["durs"])]
     size = lambda s: int(s[1] - s[0])  # noqa: E731
-    want = [len(c) for c in ref_import.grouping_module().split_by_chunk_size(spans, per_chunk * 8, size)]
-    assert [len(c) for c in SP.split_by_chunk_size(spans, per_chunk * 8, size)] == want
+    assert [len(ch) for ch in SP.split_by_chunk_size(spans, c["per_chunk"] * 8, size)] == WANT["chunk_sizes"][seed]
 
 
-_leaf = st.one_of(st.integers(-5, 5), st.floats(-2, 2, allow_nan=False), st.text(max_size=3), st.booleans(), st.none(),
-                  st.builds(lambda v, d: np.array(v, dtype=d), st.lists(st.one_of(st.floats(-3, 3, width=32), st.just(float("nan"))), max_size=5), st.sampled_from(["float32", "float64"])),
-                  st.builds(lambda v: np.array(v, dtype=np.uint8), st.lists(st.integers(0, 255), max_size=5)))  # fmt: skip
-_tree = st.recursive(_leaf, lambda kids: st.one_of(st.lists(kids, max_size=4), st.tuples(kids, kids), st.dictionaries(st.sampled_from(["a", "b", "c", 1]), kids, max_size=3)), max_leaves=12)
+def _compare_values_agrees_with_the_reference(seed):
+    c, want = RC.compare_case(seed), WANT["compare_values"][seed]
+    for (g, cand), w in zip(((c["golden"], c["candidate"]), (c["golden"], c["golden"])), want):
+        assert repr([RC.diff_key(d) for d in C.compare_values("t", g, cand, atol=c["atol"])]) == w  # repr: NaN-carrying details compare equal as text
 
 
-@_cfg
-@given(golden=_tree, candidate=_tree, atol=st.sampled_from([0.0, 1e-3, 0.5, 2.0]))
-def test_compare_values_agrees_with_the_reference(golden, candidate, atol):
-    ref = ref_import.stage_compare_functions()["_compare_values"]
-    key = lambda d: (d.field, d.detail, d.max_diff_observed, d.shape_mismatch)  # noqa: E731
-    for g, c in ((golden, candidate), (golden, golden)):
-        want, got = [key(d) for d in ref("t", g, c, atol=atol)], [key(d) for d in C.compare_values("t", g, c, atol=atol)]
-        assert repr(got) == repr(want)  # repr: NaN-carrying details compare equal as text
-
-
-@_cfg
-@given(track=st.lists(st.sampled_from([0, 0, 0, 0, 1]), min_size=1, max_size=600), entire=st.booleans(), min_len=st.one_of(st.none(), st.integers(1, 80)),
-       max_len=st.one_of(st.none(), st.integers(1, 200)), mode=st.sampled_from(["truncate", "stride"]), crop=st.one_of(st.none(), st.integers(0, 20)))
-def test_shot_logic_agrees_with_the_reference(track, entire, min_len, max_len, mode, crop):
+def _shot_logic_agrees_with_the_reference(seed):
     """0/1 transition tracks -> scenes -> filtered scenes: transnetv2_extraction_stages._get_scenes / _get_filtered_scenes."""
     from cosmos_curate_b200 import shots
 
-    f = ref_import.transnetv2_stage_functions()
-    pred = np.array(track, dtype=np.uint8).reshape(-1, 1)
-    want = f["_get_scenes"](pred, entire_scene_as_clip=entire)
-    got = shots.scenes_from_predictions(pred, entire_scene_as_clip=entire)
-    assert np.array_equal(got, want) and got.dtype == want.dtype
-    if len(want):
-        want_f = f["_get_filtered_scenes"](want.copy(), min_length=min_len, max_length=max_len, max_length_mode=mode, crop_length=crop)
-        got_f = shots.filter_scenes(got.copy(), min_length=min_len, max_length=max_len, max_length_mode=mode, crop_length=crop)
-        assert np.array_equal(got_f, want_f)
+    c, want = RC.shot_case(seed), WANT["shot_logic"][seed]
+    got = shots.scenes_from_predictions(c["track"], entire_scene_as_clip=c["entire"])
+    assert got.tolist() == want["scenes"] and str(got.dtype) == want["dtype"]
+    if want["filtered"] is not None:
+        got_f = shots.filter_scenes(got.copy(), min_length=c["min_len"], max_length=c["max_len"], max_length_mode=c["mode"], crop_length=c["crop"])
+        assert np.asarray(got_f).tolist() == want["filtered"]
 
 
-@settings(max_examples=60, deadline=None, suppress_health_check=[HealthCheck.too_slow])
-@given(h=st.integers(1, 260), w=st.integers(1, 260), th=st.integers(1, 72), tw=st.integers(1, 72), n=st.integers(8, 19), seed=st.integers(0, 2**31 - 1))
-def test_video_tube_oracle_agrees_with_the_reference_formulation(h, w, th, tw, n, seed):
+def _video_tube_oracle_agrees_with_the_reference_formulation(seed):
     """oracle/video_tube.py vs InternVideo2MultiModality._construct_frames (cv2.resize + numpy) on arbitrary sizes, every float32 bit:
     up- and down-scaling, 1-pixel sources and targets, the exact-2x INTER_AREA reroute, the copy for equal sizes."""
     from oracle import video_tube as T
 
-    rng = np.random.default_rng(seed)
-    frames = [rng.integers(0, 256, size=(h, w, 3), dtype=np.uint8) for _ in range(n)]
-    want = ref_import.internvideo2_formulator()._construct_frames(frames, fnum=8, target_size=(tw, th))
-    got = T.construct_frames(frames, fnum=8, target_size=(tw, th))
-    assert got.shape == want.shape and np.array_equal(got, want)
+    c, want = RC.video_tube_case(seed), WANT["video_tube"][seed]
+    got = T.construct_frames(c["frames"], fnum=8, target_size=c["target"])
+    assert list(got.shape) == want["shape"] and str(got.dtype) == want["dtype"]
+    assert hashlib.sha256(np.ascontiguousarray(got).tobytes()).hexdigest() == want["sha256"]
+
+
+def _all_seeds(check):
+    bad = []
+    for seed in SEEDS:
+        try:
+            check(seed)
+        except AssertionError as exc:
+            bad.append(f"seed {seed}: {str(exc)[:200]}")
+    assert not bad, "\n".join(bad)
+
+
+def test_sample_closest_agrees_with_the_reference():
+    _all_seeds(_sample_closest_agrees_with_the_reference)
+
+
+def test_fixed_stride_spans_and_uuids_agree_with_the_reference():
+    _all_seeds(_fixed_stride_spans_and_uuids_agree_with_the_reference)
+
+
+def test_chunk_sizes_agree_with_the_reference():
+    _all_seeds(_chunk_sizes_agree_with_the_reference)
+
+
+def test_compare_values_agrees_with_the_reference():
+    _all_seeds(_compare_values_agrees_with_the_reference)
+
+
+def test_shot_logic_agrees_with_the_reference():
+    _all_seeds(_shot_logic_agrees_with_the_reference)
+
+
+def test_video_tube_oracle_agrees_with_the_reference_formulation():
+    _all_seeds(_video_tube_oracle_agrees_with_the_reference_formulation)

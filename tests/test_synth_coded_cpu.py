@@ -25,8 +25,11 @@ _DECODE = textwrap.dedent(
     w, h, fps, secs, deblock = int(sys.argv[2]), int(sys.argv[3]), 30, float(sys.argv[4]), sys.argv[5] == "1"
     mp4, info = S.make_coded_clip(w, h, fps, secs, seed=int(sys.argv[6]), bitrate=float(sys.argv[7]), deblock=deblock,
                                   ac_density=0.25 if deblock else 0.0, return_info=True)
-    open("/tmp/_cb_coded.mp4", "wb").write(mp4)
-    cap = cv2.VideoCapture("/tmp/_cb_coded.mp4")
+    import tempfile
+    tmp = tempfile.NamedTemporaryFile(suffix=".mp4")
+    tmp.write(mp4)
+    tmp.flush()
+    cap = cv2.VideoCapture(tmp.name)
     cap.set(cv2.CAP_PROP_CONVERT_RGB, 0)
     pcm = info["pcm"][:256].reshape(16, 16)
     rows = h - (h // 16) * 16 or 16   # visible rows of the last macroblock row
