@@ -88,6 +88,30 @@ __device__ __forceinline__ void tma_load_2d_hint(void* dst, const CUtensorMap* m
       "l"(m), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "l"(policy)
       : "memory");
 }
+// pull a box of the tensor into L2 only (no shared memory, no barrier)
+__device__ __forceinline__ void tma_prefetch_l2_2d(const CUtensorMap* m, int c0, int c1) {
+  asm volatile("cp.async.bulk.prefetch.tensor.2d.L2.global.tile [%0, {%1, %2}];" ::"l"(m), "r"(c0), "r"(c1) : "memory");
+}
+
+// ---------------------------------------------------------------- TMA stores (shared::cta -> global), bulk async-groups
+// Boxes that reach past the tensor's extent are clipped: only the in-range elements are written. Groups are per thread: the
+// thread that commits a group is the one that waits for it.
+__device__ __forceinline__ void tma_store_2d(const CUtensorMap* m, const void* src, int c0, int c1) {
+  asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];" ::"l"(m), "r"(smem_u32(src)), "r"(c0), "r"(c1)
+               : "memory");
+}
+__device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void bulk_wait_read() {  // at most N groups still reading their shared-memory source
+  asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(N) : "memory");
+}
+template <int N>
+__device__ __forceinline__ void bulk_wait() {  // at most N groups not yet complete (writes performed)
+  asm volatile("cp.async.bulk.wait_group %0;" ::"n"(N) : "memory");
+}
+// barrier `id` (1..15; 0 is __syncthreads) over `threads` threads, a multiple of 32
+__device__ __forceinline__ void named_bar_sync(int id, int threads) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(threads) : "memory"); }
+
 __device__ __forceinline__ uint64_t policy_evict_first() {
   uint64_t p;
   asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(p));

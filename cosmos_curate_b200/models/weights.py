@@ -47,7 +47,7 @@ class VitConfig:
         return self.layers * per_layer + 2 * g2 * 3 * self.patch**2 * d + 2 * d * self.proj_dim
 
     def gemm_flops_per_image(self) -> float:
-        """The part executed by the tcgen05 GEMM kernel (everything but attention's QK^T / PV and the pooled tail)."""
+        """The part executed by the wgmma GEMM kernel (everything but attention's QK^T / PV and the pooled tail)."""
         t, d, m = self.tokens, self.hidden, self.mlp
         g2 = (self.image_size // self.patch) ** 2
         return self.layers * (2 * t * d * 3 * d + 2 * t * d * d + 2 * 2 * t * d * m) + 2 * g2 * 3 * self.patch**2 * d
