@@ -7,7 +7,7 @@
 // Persistent CTAs (one per SM) loop over (image, head) units; Q, K and V of a unit arrive by TMA into a two-deep ring.
 //
 // Warp roles (384 threads):
-//   warpgroup 0  warp 0: TMA producer (Q 32 KB, K 32 + 1 KB, V 32 + 2 KB per unit from the [n*T][3*hidden] QKV matrix)
+//   warpgroup 0  warp 0: TMA producer (Q 32 KB, K 32 + 1 KB, V 32 + 2 KB per unit from the [n][T][3*hidden] QKV tensor)
 //                warp 1: query row 256 entirely on SIMT (257 dot products of 64 + softmax + 257-term weighted sum from smem K/V)
 //   warpgroups 1-2  query rows 0..127 / 128..255, 64 at a time: S in registers (128 per thread), row max / exp2 / row sum with
 //                quad shuffles, P packed to fp16 IN PLACE as the register A operand of O = P V (the accumulator layout of S is
@@ -78,17 +78,17 @@ __global__ void __launch_bounds__(kAtThreads, 1) attention_wgmma_kernel(const __
       if (lane == 0) {  // ===== TMA producer
         int it = 0;
         for (int u = blockIdx.x; u < a.n_units; u += gridDim.x, ++it) {
-          const int img = u / a.heads, h = u - img * a.heads, row0 = img * T, s = it & 1;
+          const int img = u / a.heads, h = u - img * a.heads, s = it & 1;
           uint8_t* st = smem + s * kAtStage;
           mbar_wait_parked(&empty[s], ((it >> 1) & 1) ^ 1);
           mbar_expect_tx(&full[s], 3 * 32768 + (has_extra ? 1024 + 2048 : 0));
           for (int half = 0; half < 2; ++half) {
-            tma_load_2d(st + kAtK + half * 16384, &map_qkv, &full[s], hidden + h * 64, row0 + half * 128);
-            tma_load_2d(st + kAtQ + half * 16384, &map_qkv, &full[s], h * 64, row0 + half * 128);
+            tma_load_3d(st + kAtK + half * 16384, &map_qkv, &full[s], hidden + h * 64, half * 128, img);
+            tma_load_3d(st + kAtQ + half * 16384, &map_qkv, &full[s], h * 64, half * 128, img);
           }
-          if (has_extra) tma_load_2d(st + kAtK + 32768, &map_k8, &full[s], hidden + h * 64, row0 + 256);
-          for (int half = 0; half < 2; ++half) tma_load_2d(st + kAtV + half * 16384, &map_qkv, &full[s], 2 * hidden + h * 64, row0 + half * 128);
-          if (has_extra) tma_load_2d(st + kAtV + 32768, &map_v16, &full[s], 2 * hidden + h * 64, row0 + 256);
+          if (has_extra) tma_load_3d(st + kAtK + 32768, &map_k8, &full[s], hidden + h * 64, 256, img);
+          for (int half = 0; half < 2; ++half) tma_load_3d(st + kAtV + half * 16384, &map_qkv, &full[s], 2 * hidden + h * 64, half * 128, img);
+          if (has_extra) tma_load_3d(st + kAtV + 32768, &map_v16, &full[s], 2 * hidden + h * 64, 256, img);
         }
       }
     } else if (warp == 1) {  // ===== query row 256 on SIMT
@@ -256,15 +256,19 @@ int attention_wgmma(cb_ctx* ctx, const void* qkv, void* out, int n, int tokens, 
   if (head_dim != 64 || tokens < 129 || tokens > 257) return CB_OK;
   const int hidden = heads * 64;
   CUtensorMap map, map_k8, map_v16;
-  const uint64_t dims[2] = {(uint64_t)3 * hidden, (uint64_t)n * tokens}, strides[1] = {(uint64_t)3 * hidden * 2};
-  const uint32_t box[2] = {64, 128}, box8[2] = {64, 8}, box16[2] = {64, 16};
-  int rc = make_tensor_map(ctx, &map, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, qkv, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_128B);
+  // rank 3, {3*hidden, T, n}: a tile never reaches into the next image.  TMA zero-fills its rows past the image's own T, so the
+  // masked keys and query rows of a short image, and the rows past token 256 of the tiles below, hold zeros: P.V multiplies their
+  // zero probabilities by 0, never by a neighbouring image's V (an Inf or NaN there would turn 0 * V into NaN).
+  const uint64_t dims[3] = {(uint64_t)3 * hidden, (uint64_t)tokens, (uint64_t)n};
+  const uint64_t strides[2] = {(uint64_t)3 * hidden * 2, (uint64_t)tokens * 3 * hidden * 2};
+  const uint32_t box[3] = {64, 128, 1}, box8[3] = {64, 8, 1}, box16[3] = {64, 16, 1};
+  int rc = make_tensor_map(ctx, &map, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 3, qkv, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_128B);
   if (rc) return rc;
-  // the tiles that start at token 256: one MMA n-step of keys, one MMA k-step of values.  Their rows past token 256 belong to the
-  // next image (or are zero-filled past the end of the matrix); the kernel gives them zero probability.
-  rc = make_tensor_map(ctx, &map_k8, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, qkv, dims, strides, box8, CU_TENSOR_MAP_SWIZZLE_128B);
+  // the tiles that start at token 256: one MMA n-step of keys, one MMA k-step of values.  Only their first row is a token (256);
+  // the kernel gives the zero-filled rest zero probability.
+  rc = make_tensor_map(ctx, &map_k8, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 3, qkv, dims, strides, box8, CU_TENSOR_MAP_SWIZZLE_128B);
   if (rc) return rc;
-  rc = make_tensor_map(ctx, &map_v16, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, qkv, dims, strides, box16, CU_TENSOR_MAP_SWIZZLE_128B);
+  rc = make_tensor_map(ctx, &map_v16, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 3, qkv, dims, strides, box16, CU_TENSOR_MAP_SWIZZLE_128B);
   if (rc) return rc;
   static bool attr_done[64] = {};  // the attribute is per device: one process may drive several
   bool& attr_set = attr_done[ctx->device & 63];
