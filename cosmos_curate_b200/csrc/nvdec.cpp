@@ -229,13 +229,8 @@ int on_sequence(void* user, CUVIDEOFORMAT* f) {
   ci.ulNumOutputSurfaces = 2;
   // One context lock shared by the sessions of this device: cuvid pushes the lock's context around its own work, so a session
   // keeps working when its callbacks run on a thread whose current device is another GPU (one process, several devices; worker
-  // threads start on device 0).  Measured cost: none (16.43 vs 16.46 clips/s end to end with 12 sessions).  CB_NVDEC_CTX_LOCK=0
-  // drops it for A/B on single-GPU processes.
-  static const bool use_lock = [] {
-    const char* e = getenv("CB_NVDEC_CTX_LOCK");
-    return !(e && e[0] == '0');
-  }();
-  ci.vidLock = use_lock ? ((NvdecShared*)d->ctx->nvdec)->lock : nullptr;
+  // threads start on device 0).  Measured cost: none (16.43 vs 16.46 clips/s end to end with 12 sessions).
+  ci.vidLock = ((NvdecShared*)d->ctx->nvdec)->lock;
   const int rc = d->api->CreateDecoder(&d->dec, &ci);
   if (rc != 0) {
     d->dec = nullptr;

@@ -170,14 +170,15 @@ def test_resize_cubic_from_nv12_and_into_the_tower(ctx):
     assert rel.max() < 1e-3
 
 
-# ------------------------------------------------------------------------------------ tensor-pipe generation vs SIMT generation
+# ------------------------------------------------------------------------------------ tensor-pipe kernel vs SIMT kernel
 @pytest.mark.parametrize(("h", "w", "pitch", "res", "colour"), [(1080, 1920, 2048, 224, "opencv"), (1080, 1920, 2048, 224, "swscale"), (2160, 3840, 3840, 384, "swscale"),
                                                                 (480, 854, 1024, 224, "swscale"), (720, 1280, 1280, 384, "opencv"), (360, 640, 640, 224, "opencv"),
-                                                                (2160, 3840, 3840, 224, "swscale")])
+                                                                (2160, 3840, 3840, 224, "swscale"), (2160, 3840, 3840, 192, "opencv")])
 def test_tensor_pipe_preprocess_agrees_with_simt_kernel_and_oracle(ctx, monkeypatch, h, w, pitch, res, colour):
-    """clip_preprocess_tc_kernel (horizontal pass as a banded fp16 hi/lo GEMM on tcgen05, the default) against the v2 SIMT kernel
-    (CB_PRE_KERNEL=2) and the oracle: same u8 image within the fp32-summation-order budget, both colour conversions, 1080p -> 224
-    (bench shape), 4K -> 384 (SoViT shape, 24 vertical taps, 256-column windows), widths that are not a multiple of the window."""
+    """clip_preprocess_tc_kernel (horizontal pass as a banded fp16 hi/lo GEMM on wgmma, the default) against the SIMT kernel
+    (CB_PRE_KERNEL=simt) and the oracle: same u8 image within the fp32-summation-order budget, both colour conversions, 1080p -> 224
+    (bench shape), 4K -> 384 (SoViT shape, 24 vertical taps, 256-column windows), widths that are not a multiple of the window.
+    4K -> 192 has 45 vertical taps, more than the tensor-pipe kernel takes: there the default call falls back to the SIMT kernel."""
     from gpu_helpers import nv12_pool
 
     frames = [color.synthetic_nv12(h, w, seed=60 + s) for s in range(2)]
@@ -189,21 +190,23 @@ def test_tensor_pipe_preprocess_agrees_with_simt_kernel_and_oracle(ctx, monkeypa
     got_tc = ctx.preprocess_clip_u8(pool, res=res).cpu().numpy()
     from cosmos_curate_b200._lib import CurateB200Error
 
-    monkeypatch.setenv("CB_PRE_KERNEL", "2")
+    monkeypatch.setenv("CB_PRE_KERNEL", "simt")
     try:
-        got_v2 = ctx.preprocess_clip_u8(pool, res=res).cpu().numpy()
+        got_simt = ctx.preprocess_clip_u8(pool, res=res).cpu().numpy()
     except CurateB200Error:  # a downscale beyond the SIMT kernel's (halved) tile window
         assert (h, res) == (2160, 224)
-        got_v2 = None
+        got_simt = None
     monkeypatch.delenv("CB_PRE_KERNEL")
     conv = color.nv12_to_rgb_swscale if colour == "swscale" else color.nv12_to_rgb
     rgb = np.stack([conv(f, h, w) for f in frames])
     want = preprocess.clip_resize_crop_u8(rgb, res)
     _u8_budget(got_tc, want)
-    if got_v2 is not None:
-        _u8_budget(got_v2, want)
-        _u8_budget(got_tc, got_v2, frac=2e-4)  # two fp32 summation orders apart
-    # typed + patch outputs of the tensor-pipe path are exactly LUT(u8)
+    if got_simt is not None:
+        _u8_budget(got_simt, want)
+        _u8_budget(got_tc, got_simt, frac=2e-4)  # two fp32 summation orders apart
+    if res == 192:  # the default call ran the SIMT kernel too
+        np.testing.assert_array_equal(got_tc, got_simt)
+    # typed + patch outputs of the default path are exactly LUT(u8)
     lut = preprocess.normalize_lut()
     want32 = np.stack([lut[c][got_tc[:, c]] for c in range(3)], axis=1)
     np.testing.assert_array_equal(ctx.preprocess_clip(pool, res=res, dtype=torch.float32).cpu().numpy(), want32)

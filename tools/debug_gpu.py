@@ -1,6 +1,5 @@
 """One-off GPU diagnostics: preprocess TMA variants + first NVDEC decode.  Usage: python tools/debug_gpu.py <what>"""
 import ctypes as C
-import os
 import sys
 
 sys.path.insert(0, ".")
@@ -24,7 +23,7 @@ if what == "pre":
         torch.cuda.synchronize()
         want = preprocess.clip_resize_crop_u8(color.nv12_to_rgb(f, h, w)[None], 224)
         d = np.abs(out.astype(int) - want.astype(int))
-        print(f"variant={os.environ.get('CB_PRE_VARIANT')} {h}x{w}: maxdiff={d.max()} frac={(d>0).mean():.2e}", flush=True)
+        print(f"{h}x{w}: maxdiff={d.max()} frac={(d>0).mean():.2e}", flush=True)
 elif what == "dec":
     import cv2
 
