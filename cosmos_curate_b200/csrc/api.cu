@@ -139,14 +139,10 @@ void cb_destroy(cb_ctx* ctx) {
     cudaFree(kv.second.d_size);
     cudaFree(kv.second.d_w);
   }
-  for (auto& kv : ctx->cubic_taps) {
+  for (auto& kv : ctx->resize_taps) {
     cudaFree(kv.second.d_first);
     cudaFree(kv.second.d_wq);
     cudaFree(kv.second.d_wf);
-  }
-  for (auto& kv : ctx->linear_taps) {
-    cudaFree(kv.second.d_first);
-    cudaFree(kv.second.d_wq);
   }
   cb::release_tc_plans(ctx);
   if (ctx->d_tmp_u8) cudaFree(ctx->d_tmp_u8);

@@ -30,10 +30,10 @@ struct TapTable {  // antialiased-bicubic tap table for one axis (device memory)
   std::vector<float> h_w;          // host copy of d_w (the tensor-pipe kernel builds its fp16 hi/lo operand tiles from it)
 };
 
-struct CubicTaps {  // cv2.resize(INTER_CUBIC) tap table for one axis (device memory): 4 taps per output
+struct ResizeTaps {  // cv2.resize tap table for one axis (device memory): INTER_CUBIC (4 taps per output) or INTER_LINEAR (2)
   int* d_first = nullptr;    // [dst] source index of the first tap (unclamped)
-  short* d_wq = nullptr;     // [dst][4] weights quantised to 2^11 (OpenCV's own fixed-point path)
-  double* d_wf = nullptr;    // [dst][4] unquantised weights (IPP-style path, evaluated in double)
+  short* d_wq = nullptr;     // [dst][taps] weights quantised to 2^11 (OpenCV's own fixed-point path)
+  double* d_wf = nullptr;    // [dst][4] unquantised cubic weights (IPP-style path, evaluated in double); null for linear
 };
 
 }  // namespace cb
@@ -47,8 +47,7 @@ struct cb_ctx {
   std::mutex mu;
   PFN_cuTensorMapEncodeTiled_v12000 encode_tiled = nullptr;
   std::map<std::tuple<int, int, int, int>, cb::TapTable> taps;  // (in, out, crop_off, crop_len)
-  std::map<std::pair<int, int>, cb::CubicTaps> cubic_taps;      // (src, dst)
-  std::map<std::tuple<int, int, int>, cb::CubicTaps> linear_taps;  // (src, dst, zero fx at the borders): d_first + d_wq[dst][2]
+  std::map<std::tuple<int, int, int>, cb::ResizeTaps> resize_taps;  // (src, dst, TapKind in preprocess.cu)
   float* d_norm_lut = nullptr;                                  // [3*256] fp32, normalise LUT currently loaded
   float lut_mean[3] = {0, 0, 0}, lut_std[3] = {0, 0, 0};
   std::atomic<unsigned long long> launches{0};  // kernels launched by this library (bench.py reports it); decode threads launch too
@@ -58,7 +57,7 @@ struct cb_ctx {
   std::vector<int> prof_cat;
   size_t prof_n = 0;
   void* nvdec = nullptr;            // lazily created NVDEC state (nvdec.cpp)
-  uint8_t* d_tmp_u8 = nullptr;      // u8 [n][3][res][res] between the tensor-pipe resample kernel and the normalise/pack kernel
+  uint8_t* d_tmp_u8 = nullptr;      // u8 [n][3][res][res] between a resample kernel and the normalise/pack kernel
   size_t tmp_u8_cap = 0;
   int* d_slots = nullptr;           // device staging of the slot list of the current preprocess call
   int slots_cap = 0;
@@ -81,9 +80,10 @@ int make_tensor_map(cb_ctx* ctx, CUtensorMap* out, CUtensorMapDataType dtype, in
                     const uint64_t* strides_bytes /* rank-1 */, const uint32_t* box, CUtensorMapSwizzle swizzle);
 
 const TapTable* get_taps(cb_ctx* ctx, int in_size, int out_size, int crop_off, int crop_len);
-// preprocess_tc.cu: tensor-pipe resample (returns CB_OK, 1 = configuration not served -> use the SIMT kernel, < 0 = error)
-int run_clip_preprocess_tc(cb_ctx* ctx, const cb_surface_pool* pool, const int* d_slots, int n, int max_slot, int res, int out_mode, int patch, int k_pad,
-                           int dtype, const TapTable* tx, const TapTable* ty, void* out, cudaStream_t stream);
+// preprocess_tc.cu: tensor-pipe resample into u8 [n][3][res][res] (returns CB_OK, 1 = configuration not served -> use the SIMT kernel,
+// < 0 = error)
+int run_clip_preprocess_tc(cb_ctx* ctx, const cb_surface_pool* pool, const int* d_slots, int n, int max_slot, int res, const TapTable* tx,
+                           const TapTable* ty, uint8_t* out, cudaStream_t stream);
 void release_tc_plans(cb_ctx* ctx);
 int ensure_norm_lut(cb_ctx* ctx, const float mean[3], const float std_[3], cudaStream_t stream);
 // NV12 -> RGB -> bilinear out_w x out_h for ONE surface at `base` (used on NVDEC-mapped frames), u8 HWC into `out`.

@@ -1,17 +1,19 @@
-// Fused frame preprocess kernels (sm_90a).
+// Frame preprocess kernels (sm_90a).
 //
-//  clip_preprocess_simt_kernel : NV12 (or RGB24) frame -> YUV->RGB u8 (OpenCV BT.601 or libswscale fixed point) ->
-//      antialiased bicubic resize (ATen _upsample_bicubic2d_aa arithmetic, horizontal then vertical,
-//      fp32 FMA chains in tap order) -> centre crop -> clamp/round to u8 -> (v/255 - mean)/std LUT ->
-//      fp16/bf16/fp32, NCHW or patch-major rows for the tower's patch-embed GEMM.
-//      Replaces nvcodec_utils.py:178 + clip.py:48-62 of the reference in ONE pass over the source frame.
+//  clip_preprocess_simt_kernel : NV12 (or RGB24) frame -> YUV->RGB u8 (colour.cuh) -> antialiased bicubic resize
+//      (ATen _upsample_bicubic2d_aa arithmetic, horizontal then vertical, fp32 FMA chains in tap order) -> centre crop ->
+//      clamp/round to u8 [n][3][res][res], in one pass over the source frame (nvcodec_utils.py:178 + clip.py:48-55 of the reference).
 //      Source strips are staged into shared memory by TMA (cp.async.bulk.tensor, mbarrier double buffer);
 //      a CTA owns one frame x one tile of output columns and walks down the source rows keeping a ring
 //      of horizontally filtered rows, so every source byte is fetched once per column tile.
 //      It serves RGB inputs and the NV12 shapes that the tensor-pipe kernel (preprocess_tc.cu, the default for NV12)
 //      declines; CB_PRE_KERNEL=simt forces it for every input, which the tests use to compare the two kernels.
+//  normalize_pack_kernel / pack_patches_kernel : the u8 image of either resample kernel -> (v/255 - mean)/std LUT ->
+//      fp16/bf16/fp32 NCHW, or zero-padded patch-major rows for the tower's patch-embed GEMM (clip.py:56-62).
 //  bilinear_u8_kernel     : NV12 -> RGB -> 4-tap bilinear (half-pixel centres) -> u8 HWC (27x48 frames).
 //  nv12_to_rgb_kernel     : full-resolution NV12 -> RGB24.
+//  resize_cubic_kernel    : cv2.resize(INTER_CUBIC) of a surface's RGB image.
+//  video_tube_kernel      : cv2.resize(INTER_LINEAR) + normalise -> the video towers' fp32 input.
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
 
@@ -19,45 +21,14 @@
 #include <cmath>
 #include <cstdlib>
 #include <cstring>
+#include <type_traits>
 
+#include "colour.cuh"
 #include "common.h"
 #include "ptx.cuh"
 
 namespace cb {
 
-// OpenCV ITUR_BT_601 fixed-point constants (shift 20)
-__device__ __forceinline__ void yuv_to_rgb(int y, int u, int v, int& r, int& g, int& b) {
-  const int yy = max(y - 16, 0) * 1220542;
-  u -= 128;
-  v -= 128;
-  r = (yy + (1 << 19) + 1673527 * v) >> 20;
-  g = (yy + (1 << 19) - 852492 * v - 409993 * u) >> 20;
-  b = (yy + (1 << 19) + 2116026 * u) >> 20;
-  r = min(max(r, 0), 255);
-  g = min(max(g, 0), 255);
-  b = min(max(b, 0), 255);
-}
-
-// libswscale's unscaled yuv420p -> rgb24 converter (x86 SIMD path, libswscale/x86/yuv_2_rgb.asm; coefficients from
-// ff_yuv2rgb_c_init_tables for ITU-R BT.601 limited range, the default PyAV / cv2 leave in place): 16-bit fixed point,
-// every product truncated by pmulhw - (8Y - 128) * 9539 >> 16 etc. - nearest chroma.  This is what the reference's CPU decode
-// (decode_video_cpu_frame_ids -> frame.to_ndarray(format="rgb24"), decoder_utils.py:439-451) feeds the CLIP transforms.
-// Pinned bit-exactly against cv2/libswscale over the whole u8 range (tests/test_oracle_cpu.py).
-__device__ __forceinline__ void yuv_to_rgb_sws(int y, int u, int v, int& r, int& g, int& b) {
-  const int yy = (((y << 3) - 128) * 9539) >> 16;
-  const int uu = (u << 3) - 1024, vv = (v << 3) - 1024;
-  r = yy + ((vv * 13075) >> 16);
-  g = yy + ((uu * -3209) >> 16) + ((vv * -6660) >> 16);
-  b = yy + ((uu * 16525) >> 16);
-  r = min(max(r, 0), 255);
-  g = min(max(g, 0), 255);
-  b = min(max(b, 0), 255);
-}
-template <int FMT>
-__device__ __forceinline__ void yuv_to_rgb_fmt(int y, int u, int v, int& r, int& g, int& b) {
-  if (FMT == CB_FMT_NV12_SWS) yuv_to_rgb_sws(y, u, v, r, g, b);
-  else yuv_to_rgb(y, u, v, r, g, b);
-}
 __host__ __device__ __forceinline__ constexpr bool is_nv12(int fmt) { return fmt == CB_FMT_NV12 || fmt == CB_FMT_NV12_SWS; }
 
 constexpr int kThreads = 256;
@@ -66,7 +37,6 @@ constexpr int kSR = 32;  // source rows per strip (= lanes of a warp in the hori
 struct ClipArgs {
   const int* slots;  // device [n]
   int n, src_w, src_h, res;
-  int res_out;  // rows/columns actually emitted: res, or (res / patch) * patch for the patch layout (a stride-p conv drops the rest)
   const int *xmin, *xsize, *ymin, *ysize;  // cropped tap tables, [res]
   const float *wx, *wy;                    // [res][tx], [res][ty]
   int tx, ty;
@@ -74,19 +44,10 @@ struct ClipArgs {
   int tc;                 // output columns per CTA
   int swa;                // strip width in pixels (multiple of 16)
   int ring;               // ring rows (power of two >= kSR + ty)
-  const float* lut;       // [3][256]
-  int out_mode;           // 0 = u8 NCHW, 1 = typed NCHW, 2 = typed patch rows
   int x_align;            // source window start is aligned down to this many pixels (TMA: 16-byte aligned box start)
   int gu;                 // rows of the per-group dense weight table (>= widest 4-column union window)
-  int dtype, patch, k_pad;
-  void* out;
+  uint8_t* out;           // u8 [n][3][res][res]
 };
-
-__device__ __forceinline__ void store_typed(void* out, size_t idx, float v, int dtype) {
-  if (dtype == CB_DT_F16) ((__half*)out)[idx] = __float2half_rn(v);
-  else if (dtype == CB_DT_BF16) ((__nv_bfloat16*)out)[idx] = __float2bfloat16_rn(v);
-  else ((float*)out)[idx] = v;
-}
 
 // ------------------------------------------------------------------------------------------------ SIMT CLIP preprocess
 // Per strip of kSR source rows: colour conversion -> horizontal filter into a ring of filtered rows -> vertical filter of every
@@ -95,7 +56,7 @@ __device__ __forceinline__ void store_typed(void* out, size_t idx, float v, int 
 //     lane (= one source row) walks the UNION window once, loading each pixel once (3 x LDS.32) and applying it to
 //     the 4 columns with a dense, zero-padded weight row fetched as one broadcast LDS.128: 12 FMAs per 4 loads.
 //     fma(x, 0, acc) == acc, so the result is bit-identical to the tap-order chain.
-//   * colour conversion uses add-min-relu (DPX) instead of separate add / shift / clamp chains;
+//   * colour conversion (colour.cuh) uses add-min-relu (DPX) instead of separate add / shift / clamp chains;
 //   * all output rows that became ready in a strip are emitted in one parallel sweep.
 template <int FMT>
 __global__ void __launch_bounds__(kThreads, 2) clip_preprocess_simt_kernel(const __grid_constant__ CUtensorMap map_a,
@@ -104,7 +65,7 @@ __global__ void __launch_bounds__(kThreads, 2) clip_preprocess_simt_kernel(const
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const int frame = blockIdx.y;
   const int c0 = blockIdx.x * a.tc;
-  const int ncol = min(a.tc, a.res_out - c0);
+  const int ncol = min(a.tc, a.res - c0);
   const int slot = a.slots[frame];
   const int ngroups = (ncol + 3) >> 2;
 
@@ -116,9 +77,7 @@ __global__ void __launch_bounds__(kThreads, 2) clip_preprocess_simt_kernel(const
   float* ringb = rgbf + 3 * kSR * swp;
   float4* wg = (float4*)(((uintptr_t)(ringb + 3 * a.ring * tcp) + 15) & ~(uintptr_t)15);  // [groups][gu] x 4 columns
   int* gbase = (int*)(wg + ((a.tc + 3) >> 2) * a.gu);                                      // [groups] first source column, [groups] length
-  uint16_t* obuf = (uint16_t*)(((uintptr_t)(gbase + 2 * ((a.tc + 3) >> 2)) + 15) & ~(uintptr_t)15);
-  const int npx = (a.out_mode == 2) ? a.tc / a.patch : 0;
-  uint64_t* bars = (uint64_t*)(((uintptr_t)(obuf + npx * a.k_pad) + 7) & ~(uintptr_t)7);
+  uint64_t* bars = (uint64_t*)(((uintptr_t)(gbase + 2 * ((a.tc + 3) >> 2)) + 7) & ~(uintptr_t)7);
 
   const int x_lo = a.xmin[c0] & ~(a.x_align - 1);
 
@@ -129,8 +88,6 @@ __global__ void __launch_bounds__(kThreads, 2) clip_preprocess_simt_kernel(const
   }
   // dense weight table of this column tile
   for (int i = tid; i < ngroups * a.gu; i += kThreads) wg[i] = make_float4(0.f, 0.f, 0.f, 0.f);
-  if (a.out_mode == 2)
-    for (int i = tid; i < npx * a.k_pad; i += kThreads) obuf[i] = 0;
   __syncthreads();
   if (tid < ngroups) {
     const int cfirst = c0 + 4 * tid, base = a.xmin[cfirst];
@@ -177,10 +134,10 @@ __global__ void __launch_bounds__(kThreads, 2) clip_preprocess_simt_kernel(const
 
     // ---- phase 1: colour conversion; one thread owns a 2-row x 4-pixel block (two chroma samples, three 32-bit loads)
     if (is_nv12(FMT)) {
+      using Colour = std::conditional_t<FMT == CB_FMT_NV12_SWS, ColourSws, ColourOpenCv>;
       const int q4 = a.swa >> 2;
       const uint8_t* ry = rs;
       const uint8_t* ruv = rs + a.swa * kSR;
-      constexpr int kMax = (256 << 20) - 1;
       for (int i = tid; i < (kSR / 2) * q4; i += kThreads) {
         const int rp = i / q4, x = (i - rp * q4) * 4, r = rp * 2;
         const uint32_t ya = *(const uint32_t*)(ry + r * a.swa + x), yb = *(const uint32_t*)(ry + (r + 1) * a.swa + x);
@@ -188,35 +145,18 @@ __global__ void __launch_bounds__(kThreads, 2) clip_preprocess_simt_kernel(const
         float* p = rgbf + r * swp + x;
 #pragma unroll
         for (int h = 0; h < 2; ++h) {  // the two chroma samples of the block
-          if (FMT == CB_FMT_NV12_SWS) {  // swscale arithmetic (see yuv_to_rgb_sws): truncating 16-bit products, clamp 0..255
-            const int uu = ((int)((uv4 >> (16 * h)) & 0xff) << 3) - 1024, vv = ((int)((uv4 >> (16 * h + 8)) & 0xff) << 3) - 1024;
-            const int ruv_ = (vv * 13075) >> 16, guv_ = ((uu * -3209) >> 16) + ((vv * -6660) >> 16), buv_ = (uu * 16525) >> 16;
-#pragma unroll
-            for (int rr = 0; rr < 2; ++rr) {
-              const uint32_t yw = rr ? yb : ya;
-#pragma unroll
-              for (int k = 0; k < 2; ++k) {
-                const int yv = ((((int)((yw >> (16 * h + 8 * k)) & 0xff) << 3) - 128) * 9539) >> 16;
-                float* q = p + rr * swp + 2 * h + k;
-                q[0] = (float)__viaddmin_s32_relu(yv, ruv_, 255);
-                q[kSR * swp] = (float)__viaddmin_s32_relu(yv, guv_, 255);
-                q[2 * kSR * swp] = (float)__viaddmin_s32_relu(yv, buv_, 255);
-              }
-            }
-            continue;
-          }
-          const int u = (int)((uv4 >> (16 * h)) & 0xff) - 128, v = (int)((uv4 >> (16 * h + 8)) & 0xff) - 128;
-          const int ruv_ = 1673527 * v, guv_ = -852492 * v - 409993 * u, buv_ = 2116026 * u;
+          int ruv_, guv_, buv_;
+          Colour::chroma((int)((uv4 >> (16 * h)) & 0xff), (int)((uv4 >> (16 * h + 8)) & 0xff), ruv_, guv_, buv_);
 #pragma unroll
           for (int rr = 0; rr < 2; ++rr) {
             const uint32_t yw = rr ? yb : ya;
 #pragma unroll
             for (int k = 0; k < 2; ++k) {
-              const int yv = max((int)((yw >> (16 * h + 8 * k)) & 0xff) - 16, 0) * 1220542 + (1 << 19);
+              const int yv = Colour::luma((int)((yw >> (16 * h + 8 * k)) & 0xff));
               float* q = p + rr * swp + 2 * h + k;
-              q[0] = (float)(__viaddmin_s32_relu(yv, ruv_, kMax) >> 20);
-              q[kSR * swp] = (float)(__viaddmin_s32_relu(yv, guv_, kMax) >> 20);
-              q[2 * kSR * swp] = (float)(__viaddmin_s32_relu(yv, buv_, kMax) >> 20);
+              q[0] = (float)Colour::combine(yv, ruv_);
+              q[kSR * swp] = (float)Colour::combine(yv, guv_);
+              q[2 * kSR * swp] = (float)Colour::combine(yv, buv_);
             }
           }
         }
@@ -263,82 +203,133 @@ __global__ void __launch_bounds__(kThreads, 2) clip_preprocess_simt_kernel(const
     }
     __syncthreads();
 
-    // ---- phase 3: emit all output rows whose vertical window is complete, one patch row at a time
+    // ---- phase 3: emit all output rows whose vertical window is complete, one warp per output row, lane = column
     int last = next_out;
     const bool final_strip = (s == a.n_strips - 1);
-    while (last < a.res_out && (final_strip || a.ymin[last] + a.ysize[last] <= y0 + kSR)) ++last;
-    int seg = next_out;
-    while (seg < last) {
-      const int seg_end = (a.out_mode == 2) ? min(last, (seg / a.patch + 1) * a.patch) : last;
-      for (int yo = seg + warp; yo < seg_end; yo += kThreads / 32) {  // one warp per output row, lane = column
-        const int ym = a.ymin[yo], ys = a.ysize[yo];
-        const float* wrow = a.wy + (size_t)yo * a.ty;
-        const float w_lo = lane < ys ? __ldg(wrow + lane) : 0.f, w_hi = lane + 32 < ys ? __ldg(wrow + lane + 32) : 0.f;
-        const int c = min(lane, ncol - 1);
-        const float* rb = ringb + c;
-        const int chs = a.ring * tcp;
-        float acc0 = 0.f, acc1 = 0.f, acc2 = 0.f;
-        for (int k = 0; k < ys; ++k) {
-          const float w = __shfl_sync(0xffffffffu, k < 32 ? w_lo : w_hi, k & 31);
-          const float* rr = rb + ((ym + k) & (a.ring - 1)) * tcp;
-          acc0 = fmaf(rr[0], w, acc0), acc1 = fmaf(rr[chs], w, acc1), acc2 = fmaf(rr[2 * chs], w, acc2);
-        }
-        if (lane < ncol) {
-          const int x = c0 + c;
+    while (last < a.res && (final_strip || a.ymin[last] + a.ysize[last] <= y0 + kSR)) ++last;
+    for (int yo = next_out + warp; yo < last; yo += kThreads / 32) {
+      const int ym = a.ymin[yo], ys = a.ysize[yo];
+      const float* wrow = a.wy + (size_t)yo * a.ty;
+      const float w_lo = lane < ys ? __ldg(wrow + lane) : 0.f, w_hi = lane + 32 < ys ? __ldg(wrow + lane + 32) : 0.f;
+      const int c = min(lane, ncol - 1);
+      const float* rb = ringb + c;
+      const int chs = a.ring * tcp;
+      float acc0 = 0.f, acc1 = 0.f, acc2 = 0.f;
+      for (int k = 0; k < ys; ++k) {
+        const float w = __shfl_sync(0xffffffffu, k < 32 ? w_lo : w_hi, k & 31);
+        const float* rr = rb + ((ym + k) & (a.ring - 1)) * tcp;
+        acc0 = fmaf(rr[0], w, acc0), acc1 = fmaf(rr[chs], w, acc1), acc2 = fmaf(rr[2 * chs], w, acc2);
+      }
+      if (lane < ncol) {
 #pragma unroll
-          for (int ch = 0; ch < 3; ++ch) {
-            float acc = ch == 0 ? acc0 : (ch == 1 ? acc1 : acc2);
-            acc = fminf(fmaxf(acc, 0.f), 255.f);
-            const int v = __float2int_rn(acc);
-            if (a.out_mode == 0) {
-              ((uint8_t*)a.out)[(((size_t)frame * 3 + ch) * a.res + yo) * a.res + x] = (uint8_t)v;
-            } else {
-              const float f = a.lut[ch * 256 + v];
-              if (a.out_mode == 1) {
-                store_typed(a.out, (((size_t)frame * 3 + ch) * a.res + yo) * a.res + x, f, a.dtype);
-              } else {
-                const int ip = c / a.patch, px_ = c - ip * a.patch, py = yo % a.patch;
-                const uint16_t bits = (a.dtype == CB_DT_F16) ? __half_as_ushort(__float2half_rn(f))
-                                                             : __bfloat16_as_ushort(__float2bfloat16_rn(f));
-                obuf[ip * a.k_pad + (ch * a.patch + py) * a.patch + px_] = bits;
-              }
-            }
-          }
+        for (int ch = 0; ch < 3; ++ch) {
+          const float acc = ch == 0 ? acc0 : (ch == 1 ? acc1 : acc2);
+          a.out[(((size_t)frame * 3 + ch) * a.res + yo) * a.res + c0 + c] = (uint8_t)__float2int_rn(fminf(fmaxf(acc, 0.f), 255.f));
         }
       }
-      if (a.out_mode == 2 && (seg_end % a.patch) == 0) {  // a row of patches is complete: 128-bit stores
-        __syncthreads();
-        const int gsz = a.res / a.patch, prow = (seg_end - 1) / a.patch, vec = a.k_pad >> 3;
-        const int np = ncol / a.patch;
-        for (int i = tid; i < np * vec; i += kThreads) {
-          const int ip = i / vec, q = i - ip * vec;
-          uint4* dst = (uint4*)((uint16_t*)a.out + ((size_t)frame * gsz * gsz + (size_t)prow * gsz + (c0 / a.patch + ip)) * a.k_pad);
-          dst[q] = ((const uint4*)(obuf + ip * a.k_pad))[q];
-        }
-        __syncthreads();
-      }
-      seg = seg_end;
     }
     next_out = last;
   }
 }
 #undef CB_ISSUE_STRIP
 
-// ------------------------------------------------------------------------------------------------
-struct SimpleArgs {
-  const uint8_t* base;
-  size_t slot_stride;
-  const int* slots;
-  int n, w, h, pitch, luma_rows, out_w, out_h, format;
-  uint8_t* out;
+// ------------------------------------------------------------------------------------------------ normalise / pack
+// u8 [n][3][res][res] -> normalised output: typed NCHW, or zero-padded patch rows [n][(res/p)^2][k_pad]
+struct PackArgs {
+  const uint8_t* src;
+  const float* lut;  // [3][256]
+  int n, res, dtype, patch, k_pad;
+  void* out;
 };
 
-__device__ __forceinline__ void fetch_rgb_nv12(const uint8_t* f, int pitch, int luma_rows, int x, int y, int& r, int& g, int& b, int format = CB_FMT_NV12) {
-  const int Y = f[(size_t)y * pitch + x];
-  const uint8_t* uv = f + (size_t)luma_rows * pitch + (size_t)(y >> 1) * pitch + (x & ~1);
-  if (format == CB_FMT_NV12_SWS) yuv_to_rgb_sws(Y, uv[0], uv[1], r, g, b);
-  else yuv_to_rgb(Y, uv[0], uv[1], r, g, b);
+__device__ __forceinline__ void store_out(void* out, size_t idx, float v, int dtype) {
+  if (dtype == CB_DT_F16) reinterpret_cast<__half*>(out)[idx] = __float2half_rn(v);
+  else if (dtype == CB_DT_BF16) reinterpret_cast<__nv_bfloat16*>(out)[idx] = __float2bfloat16_rn(v);
+  else reinterpret_cast<float*>(out)[idx] = v;
 }
+
+__global__ void normalize_pack_kernel(const PackArgs a) {  // typed NCHW, one element per thread (parity-test output)
+  const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  const size_t plane = (size_t)a.res * a.res;
+  if (i >= 3 * plane * a.n) return;
+  const int ch = (int)((i / plane) % 3);
+  store_out(a.out, i, a.lut[ch * 256 + a.src[i]], a.dtype);
+}
+
+// Patch rows: one CTA per (frame, patch row): the k -> (plane, y, x) map of a patch is built once in shared memory, then every thread
+// emits 8 consecutive elements of a zero-padded patch row per iteration as one 16-byte store.
+__global__ void __launch_bounds__(256) pack_patches_kernel(const PackArgs a) {
+  extern __shared__ int koff[];  // [kz]: (plane << 24) | offset inside the patch origin's plane, -1 = padding
+  const int g = a.res / a.patch, pp = a.patch * a.patch;
+  const int kz = (3 * pp + 7) & ~7;  // the patch's elements in whole 16-byte stores; the stores past kz are all padding
+  for (int k = threadIdx.x; k < kz; k += blockDim.x) {
+    int v = -1;
+    if (k < 3 * pp) {
+      const int ch = k / pp, yy = (k - ch * pp) / a.patch, xx = k - ch * pp - yy * a.patch;
+      v = (ch << 24) | (yy * a.res + xx);
+    }
+    koff[k] = v;
+  }
+  __syncthreads();
+  const int py = blockIdx.x, f = blockIdx.y;
+  const size_t plane = (size_t)a.res * a.res;
+  const uint8_t* img = a.src + (size_t)f * 3 * plane + (size_t)py * a.patch * a.res;
+  const int k8 = a.k_pad >> 3;
+  const bool bf = a.dtype == CB_DT_BF16;
+  for (int i = threadIdx.x; i < g * k8; i += blockDim.x) {
+    const int px = i / k8, kk = (i - px * k8) << 3;
+    uint32_t w[4] = {0, 0, 0, 0};
+    if (kk < kz) {
+#pragma unroll
+      for (int e = 0; e < 4; ++e) {
+        float v[2];
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const int o = koff[kk + 2 * e + h];
+          const int ch = o >> 24;
+          v[h] = o < 0 ? 0.f : a.lut[ch * 256 + img[(size_t)ch * plane + (o & 0xFFFFFF) + px * a.patch]];
+        }
+        if (bf) {
+          __nv_bfloat162 b = __floats2bfloat162_rn(v[0], v[1]);
+          w[e] = *reinterpret_cast<uint32_t*>(&b);
+        } else {
+          __half2 hh = __floats2half2_rn(v[0], v[1]);
+          w[e] = *reinterpret_cast<uint32_t*>(&hh);
+        }
+      }
+    }
+    uint4* dst = reinterpret_cast<uint4*>(reinterpret_cast<uint16_t*>(a.out) + (((size_t)f * g + py) * g + px) * a.k_pad + kk);
+    *dst = make_uint4(w[0], w[1], w[2], w[3]);
+  }
+}
+
+// ------------------------------------------------------------------------------------------------ per-pixel surface kernels
+struct Surface {  // a cb_surface_pool as the per-pixel kernels read it
+  const uint8_t* base;
+  size_t slot_stride;
+  const int* slots;  // device [n]; null: frame f is the surface at base + f * slot_stride
+  int w, h, pitch, luma_rows, format;
+
+  __device__ __forceinline__ const uint8_t* frame(int f) const { return base + (size_t)(slots ? slots[f] : f) * slot_stride; }
+  // RGB of pixel (x, y) of a frame: NV12 through the pool's colour arithmetic (nearest chroma), or RGB24
+  __device__ __forceinline__ void rgb(const uint8_t* fr, int x, int y, int& r, int& g, int& b) const {
+    if (!is_nv12(format)) {
+      const uint8_t* px = fr + (size_t)y * pitch + 3 * x;
+      r = px[0], g = px[1], b = px[2];
+      return;
+    }
+    const int Y = fr[(size_t)y * pitch + x];
+    const uint8_t* uv = fr + (size_t)luma_rows * pitch + (size_t)(y >> 1) * pitch + (x & ~1);
+    if (format == CB_FMT_NV12_SWS) yuv_to_rgb<ColourSws>(Y, uv[0], uv[1], r, g, b);
+    else yuv_to_rgb<ColourOpenCv>(Y, uv[0], uv[1], r, g, b);
+  }
+};
+
+struct SimpleArgs {
+  Surface s;
+  int n, out_w, out_h;
+  uint8_t* out;
+};
 
 // cvcuda.resize_into(LINEAR) semantics: half-pixel centres, clamp-to-edge taps, fp32, round-to-nearest-even.
 __global__ void bilinear_u8_kernel(const SimpleArgs a) {
@@ -346,18 +337,19 @@ __global__ void bilinear_u8_kernel(const SimpleArgs a) {
   const int per = a.out_w * a.out_h;
   if (i >= a.n * per) return;
   const int f = i / per, p = i - f * per, yo = p / a.out_w, xo = p - yo * a.out_w;
-  const uint8_t* fr = a.base + (size_t)(a.slots ? a.slots[f] : f) * a.slot_stride;
-  const float sx = (float)a.w / (float)a.out_w, sy = (float)a.h / (float)a.out_h;
+  const Surface& s = a.s;
+  const uint8_t* fr = s.frame(f);
+  const float sx = (float)s.w / (float)a.out_w, sy = (float)s.h / (float)a.out_h;
   const float fx = (xo + 0.5f) * sx - 0.5f, fy = (yo + 0.5f) * sy - 0.5f;
   const int x0 = (int)floorf(fx), y0 = (int)floorf(fy);
   const float wx = fx - (float)x0, wy = fy - (float)y0;
-  const int xa = min(max(x0, 0), a.w - 1), xb = min(max(x0 + 1, 0), a.w - 1);
-  const int ya = min(max(y0, 0), a.h - 1), yb = min(max(y0 + 1, 0), a.h - 1);
+  const int xa = min(max(x0, 0), s.w - 1), xb = min(max(x0 + 1, 0), s.w - 1);
+  const int ya = min(max(y0, 0), s.h - 1), yb = min(max(y0 + 1, 0), s.h - 1);
   int p00[3], p01[3], p10[3], p11[3];
-  fetch_rgb_nv12(fr, a.pitch, a.luma_rows, xa, ya, p00[0], p00[1], p00[2], a.format);
-  fetch_rgb_nv12(fr, a.pitch, a.luma_rows, xb, ya, p01[0], p01[1], p01[2], a.format);
-  fetch_rgb_nv12(fr, a.pitch, a.luma_rows, xa, yb, p10[0], p10[1], p10[2], a.format);
-  fetch_rgb_nv12(fr, a.pitch, a.luma_rows, xb, yb, p11[0], p11[1], p11[2], a.format);
+  s.rgb(fr, xa, ya, p00[0], p00[1], p00[2]);
+  s.rgb(fr, xb, ya, p01[0], p01[1], p01[2]);
+  s.rgb(fr, xa, yb, p10[0], p10[1], p10[2]);
+  s.rgb(fr, xb, yb, p11[0], p11[1], p11[2]);
 #pragma unroll
   for (int ch = 0; ch < 3; ++ch) {
     const float top = __fadd_rn(__fmul_rn((float)p00[ch], 1.f - wx), __fmul_rn((float)p01[ch], wx));
@@ -370,25 +362,21 @@ __global__ void bilinear_u8_kernel(const SimpleArgs a) {
 
 __global__ void nv12_to_rgb_kernel(const SimpleArgs a) {
   // one thread per horizontal pixel pair; out tightly packed [n][h][w][3]
-  const int pairs_w = (a.w + 1) >> 1;
-  const size_t per = (size_t)pairs_w * a.h;
+  const Surface& s = a.s;
+  const int pairs_w = (s.w + 1) >> 1;
+  const size_t per = (size_t)pairs_w * s.h;
   const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= per * a.n) return;
   const int f = (int)(i / per);
   const size_t p = i - (size_t)f * per;
   const int y = (int)(p / pairs_w), x = (int)(p - (size_t)y * pairs_w) * 2;
-  const uint8_t* fr = a.base + (size_t)a.slots[f] * a.slot_stride;
-  const uint8_t* uv = fr + (size_t)a.luma_rows * a.pitch + (size_t)(y >> 1) * a.pitch + x;
-  const int U = uv[0], V = uv[1];
-  uint8_t* o = a.out + (((size_t)f * a.h + y) * a.w + x) * 3;
+  const uint8_t* fr = s.frame(f);
+  uint8_t* o = a.out + (((size_t)f * s.h + y) * s.w + x) * 3;
   int r, g, b;
-  const bool sws = a.format == CB_FMT_NV12_SWS;
-  if (sws) yuv_to_rgb_sws(fr[(size_t)y * a.pitch + x], U, V, r, g, b);
-  else yuv_to_rgb(fr[(size_t)y * a.pitch + x], U, V, r, g, b);
+  s.rgb(fr, x, y, r, g, b);
   o[0] = r, o[1] = g, o[2] = b;
-  if (x + 1 < a.w) {
-    if (sws) yuv_to_rgb_sws(fr[(size_t)y * a.pitch + x + 1], U, V, r, g, b);
-    else yuv_to_rgb(fr[(size_t)y * a.pitch + x + 1], U, V, r, g, b);
+  if (x + 1 < s.w) {
+    s.rgb(fr, x + 1, y, r, g, b);
     o[3] = r, o[4] = g, o[5] = b;
   }
 }
@@ -405,10 +393,8 @@ __global__ void nv12_to_rgb_kernel(const SimpleArgs a) {
 //                     noise (measured: differs from exact arithmetic on < 3e-5 of the pixels, always at ties): unquantised
 //                     weights and accumulation in double (fp32 accumulation alone flips ~3e-4 of the pixels), round half even.
 struct CubicArgs {
-  const uint8_t* base;
-  size_t slot_stride;
-  const int* slots;
-  int n, w, h, pitch, luma_rows, format, out_w, out_h, mode, n_vec;
+  Surface s;
+  int n, out_w, out_h, mode, n_vec;
   const int *x0, *y0;
   const short *wxq, *wyq;
   const double *wxf, *wyf;
@@ -420,25 +406,20 @@ __global__ void resize_cubic_kernel(const CubicArgs a) {
   const int per = a.out_w * a.out_h;
   if (i >= a.n * per) return;
   const int f = i / per, p = i - f * per, yo = p / a.out_w, xo = p - yo * a.out_w;
-  const uint8_t* fr = a.base + (size_t)a.slots[f] * a.slot_stride;
+  const uint8_t* fr = a.s.frame(f);
   const int xs = a.x0[xo], ys = a.y0[yo];
   int hs[4][3];
   double hf[4][3];  // IPP variant in double: fp32 accumulation alone moves ~3e-4 of the pixels across a rounding tie (measured)
 #pragma unroll
   for (int ky = 0; ky < 4; ++ky) {
-    const int y = min(max(ys + ky, 0), a.h - 1);
+    const int y = min(max(ys + ky, 0), a.s.h - 1);
     int acc[3] = {0, 0, 0};
     double accf[3] = {0.0, 0.0, 0.0};
 #pragma unroll
     for (int kx = 0; kx < 4; ++kx) {
-      const int x = min(max(xs + kx, 0), a.w - 1);
+      const int x = min(max(xs + kx, 0), a.s.w - 1);
       int r, g, b;
-      if (is_nv12(a.format)) {
-        fetch_rgb_nv12(fr, a.pitch, a.luma_rows, x, y, r, g, b, a.format);
-      } else {
-        const uint8_t* px = fr + (size_t)y * a.pitch + 3 * x;
-        r = px[0], g = px[1], b = px[2];
-      }
+      a.s.rgb(fr, x, y, r, g, b);
       if (a.mode == CB_CUBIC_OPENCV) {
         const int wq = a.wxq[xo * 4 + kx];
         acc[0] += r * wq, acc[1] += g * wq, acc[2] += b * wq;
@@ -489,25 +470,14 @@ __global__ void resize_cubic_kernel(const CubicArgs a) {
 // in int32, vertical pass (((b0 * (S0 >> 4)) >> 16) + ((b1 * (S1 >> 4)) >> 16) + 2) >> 2; an exact 2x2 decimation is what
 // cv2 reroutes to INTER_AREA ((a + b + c + d + 2) >> 2); equal sizes copy.  HBM-bound and sparse: 4 source pixels per output.
 struct TubeArgs {
-  const uint8_t* base;
-  size_t slot_stride;
-  const int* slots;
-  int n, w, h, pitch, luma_rows, format, out_w, out_h, mode;  // mode 0 linear, 1 area 2x2, 2 copy
+  Surface s;
+  int n, out_w, out_h, mode;  // mode 0 linear, 1 area 2x2, 2 copy
   const int *x0, *y0;
   const short *ax, *by;
   float mean[3], std_[3];
   float* out_f32;    // [n][3][out_h][out_w] or null
   uint8_t* out_u8;   // [n][out_h][out_w][3] or null
 };
-
-__device__ __forceinline__ void fetch_rgb_any(const TubeArgs& a, const uint8_t* fr, int x, int y, int& r, int& g, int& b) {
-  if (is_nv12(a.format)) {
-    fetch_rgb_nv12(fr, a.pitch, a.luma_rows, x, y, r, g, b, a.format);
-  } else {
-    const uint8_t* px = fr + (size_t)y * a.pitch + 3 * x;
-    r = px[0], g = px[1], b = px[2];
-  }
-}
 
 __global__ void video_tube_kernel(const TubeArgs a) {
   __shared__ float lut[3][256];
@@ -520,29 +490,29 @@ __global__ void video_tube_kernel(const TubeArgs a) {
   const int per = a.out_w * a.out_h;
   if (i >= a.n * per) return;
   const int f = i / per, p = i - f * per, yo = p / a.out_w, xo = p - yo * a.out_w;
-  const uint8_t* fr = a.base + (size_t)a.slots[f] * a.slot_stride;
+  const uint8_t* fr = a.s.frame(f);
   int v[3];
   if (a.mode == 2) {
-    fetch_rgb_any(a, fr, xo, yo, v[0], v[1], v[2]);
+    a.s.rgb(fr, xo, yo, v[0], v[1], v[2]);
   } else if (a.mode == 1) {
     int s[3] = {2, 2, 2};
 #pragma unroll
     for (int k = 0; k < 4; ++k) {
       int r, g, b;
-      fetch_rgb_any(a, fr, 2 * xo + (k & 1), 2 * yo + (k >> 1), r, g, b);
+      a.s.rgb(fr, 2 * xo + (k & 1), 2 * yo + (k >> 1), r, g, b);
       s[0] += r, s[1] += g, s[2] += b;
     }
     v[0] = s[0] >> 2, v[1] = s[1] >> 2, v[2] = s[2] >> 2;
   } else {
     const int xs = a.x0[xo], ys = a.y0[yo];
-    const int xa = min(max(xs, 0), a.w - 1), xb = min(max(xs + 1, 0), a.w - 1);
-    const int ya = min(max(ys, 0), a.h - 1), yb = min(max(ys + 1, 0), a.h - 1);
+    const int xa = min(max(xs, 0), a.s.w - 1), xb = min(max(xs + 1, 0), a.s.w - 1);
+    const int ya = min(max(ys, 0), a.s.h - 1), yb = min(max(ys + 1, 0), a.s.h - 1);
     const int a0 = a.ax[2 * xo], a1 = a.ax[2 * xo + 1], b0 = a.by[2 * yo], b1 = a.by[2 * yo + 1];
     int p00[3], p01[3], p10[3], p11[3];
-    fetch_rgb_any(a, fr, xa, ya, p00[0], p00[1], p00[2]);
-    fetch_rgb_any(a, fr, xb, ya, p01[0], p01[1], p01[2]);
-    fetch_rgb_any(a, fr, xa, yb, p10[0], p10[1], p10[2]);
-    fetch_rgb_any(a, fr, xb, yb, p11[0], p11[1], p11[2]);
+    a.s.rgb(fr, xa, ya, p00[0], p00[1], p00[2]);
+    a.s.rgb(fr, xb, ya, p01[0], p01[1], p01[2]);
+    a.s.rgb(fr, xa, yb, p10[0], p10[1], p10[2]);
+    a.s.rgb(fr, xb, yb, p11[0], p11[1], p11[2]);
 #pragma unroll
     for (int c = 0; c < 3; ++c) {
       const int s0 = p00[c] * a0 + p01[c] * a1, s1 = p10[c] * a0 + p11[c] * a1;
@@ -559,6 +529,7 @@ __global__ void video_tube_kernel(const TubeArgs a) {
     for (int c = 0; c < 3; ++c) o[(size_t)c * per] = lut[c][v[c] & 255];
   }
 }
+
 
 // ------------------------------------------------------------------------------------------------ host
 static float cubic_aa(float x) {  // Keys a = -0.5, float32 like ATen's bicubic_filter
@@ -667,44 +638,36 @@ static int check_pool(cb_ctx* ctx, const cb_surface_pool* pool, int n, const int
   return CB_OK;
 }
 
-// SIMT kernel: column tiles, tensor maps and launch.  run_clip_preprocess has checked the request, built the tap tables and uploaded
-// the slots and the normalisation LUT.
-static int run_clip_preprocess_simt(cb_ctx* ctx, const cb_surface_pool* pool, const int* d_slots, int n, int max_slot, int res, int out_mode,
-                                    int layout_patch, int k_pad, int dtype, const TapTable* tx, const TapTable* ty, void* out, cudaStream_t stream) {
+// SIMT kernel: column tiles, tensor maps and launch, into u8 `out` [n][3][res][res].  run_clip_preprocess has checked the request,
+// built the tap tables and uploaded the slots.
+static int run_clip_preprocess_simt(cb_ctx* ctx, const cb_surface_pool* pool, const int* d_slots, int n, int max_slot, int res, const TapTable* tx,
+                                    const TapTable* ty, uint8_t* out, cudaStream_t stream) {
   const int W = pool->width, H = pool->height;
   ClipArgs a{};
   a.slots = d_slots, a.n = n, a.src_w = W, a.src_h = H, a.res = res;
   a.xmin = tx->d_min, a.xsize = tx->d_size, a.wx = tx->d_w, a.tx = tx->max_taps;
   a.ymin = ty->d_min, a.ysize = ty->d_size, a.wy = ty->d_w, a.ty = ty->max_taps;
-  a.lut = ctx->d_norm_lut;
-  a.out_mode = out_mode, a.dtype = dtype, a.patch = layout_patch, a.k_pad = k_pad, a.out = out;
-  if (out_mode == 2) {
-    a.tc = layout_patch * (32 / layout_patch);
-    a.res_out = (res / layout_patch) * layout_patch;
-  } else {
-    a.tc = 32;
-    a.res_out = res;
-  }
+  a.out = out;
   a.y_begin = ty->src_begin & ~1;
   a.n_strips = (ty->src_end - a.y_begin + kSR - 1) / kSR;
   int ring = 64;
   while (ring < kSR + ty->max_taps) ring <<= 1;
   a.ring = ring;
   a.x_align = 16;  // cp.async.bulk.tensor needs the box to start on a 16-byte boundary of the innermost dimension
-  // widest source span of any column tile; strong downscales (4K -> 224: 9.6 source pixels per output column) halve the tile so that
-  // the window still fits one TMA box (256 bytes of the innermost dimension)
+  // widest source span of any column tile; strong downscales (4K -> 224: 9.6 source pixels per output column) narrow the tile
+  // (32 -> 16 -> 8 columns) so that the window still fits one TMA box (256 bytes of the innermost dimension).  Under the 64-tap limit
+  // an 8-column window spans at most ~200 source columns.
   int span = 0, tiles = 0;
-  for (int attempt = 0; attempt < 2; ++attempt) {
+  for (a.tc = 32;; a.tc /= 2) {
     span = 0;
-    tiles = (a.res_out + a.tc - 1) / a.tc;
+    tiles = (res + a.tc - 1) / a.tc;
     for (int t = 0; t < tiles; ++t) {
-      const int c0 = t * a.tc, c1 = std::min(a.res_out, c0 + a.tc);
+      const int c0 = t * a.tc, c1 = std::min(res, c0 + a.tc);
       int lo = tx->h_min[c0] & ~(a.x_align - 1), hi = 0;
       for (int c = c0; c < c1; ++c) hi = std::max(hi, tx->h_min[c] + tx->h_size[c]);
       span = std::max(span, hi - lo);
     }
-    if (span <= 256 || attempt == 1) break;
-    a.tc = out_mode == 2 ? layout_patch * std::max(1, 16 / layout_patch) : 16;
+    if (span <= 256 || a.tc == 8) break;
   }
   a.swa = (span + 15) & ~15;
   // widest union window of any group of 4 adjacent output columns
@@ -741,11 +704,10 @@ static int run_clip_preprocess_simt(cb_ctx* ctx, const cb_surface_pool* pool, co
   }
 
   const int raw_stage = is_nv12(pool->format) ? (a.swa * kSR * 3 / 2) : (3 * a.swa * kSR);
-  const int npx = out_mode == 2 ? a.tc / a.patch : 0;
   const int groups = (a.tc + 3) / 4;
-  // the kernel's carve-up in order; 80 bytes cover the two mbarriers and the alignment of the weight table, obuf and the barriers
+  // the kernel's carve-up in order; 80 bytes cover the two mbarriers and the alignment of the weight table and the barriers
   const size_t smem = 2 * (size_t)raw_stage + (size_t)3 * kSR * (a.swa + 1) * 4 + (size_t)3 * a.ring * (a.tc | 1) * 4 + (size_t)groups * a.gu * 16 +
-                      (size_t)2 * groups * 4 + (size_t)npx * k_pad * 2 + 80;
+                      (size_t)2 * groups * 4 + 80;
   if (smem > 227 * 1024) return fail(ctx, CB_ERR_UNSUPPORTED, "preprocess tile needs %zu bytes of shared memory", smem);
   const auto kernel = pool->format == CB_FMT_NV12       ? clip_preprocess_simt_kernel<CB_FMT_NV12>
                       : pool->format == CB_FMT_NV12_SWS ? clip_preprocess_simt_kernel<CB_FMT_NV12_SWS>
@@ -757,8 +719,10 @@ static int run_clip_preprocess_simt(cb_ctx* ctx, const cb_surface_pool* pool, co
   return CB_OK;
 }
 
-// Checks the request, builds the tap tables and uploads the normalisation LUT and the slots, then runs the tensor-pipe kernel
-// (preprocess_tc.cu) when it serves the input and the SIMT kernel otherwise.  CB_PRE_KERNEL=simt forces the SIMT kernel.
+// Checks the request, builds the tap tables and uploads the normalisation LUT and the slots, then resamples to u8 [n][3][res][res]
+// with the tensor-pipe kernel (preprocess_tc.cu) when it serves the input and with the SIMT kernel otherwise; CB_PRE_KERNEL=simt
+// forces the SIMT kernel.  out_mode 0 resamples straight into `out`.  Otherwise the u8 image goes to ctx->d_tmp_u8 and the
+// normalise/pack step writes typed NCHW (out_mode 1) or patch rows (out_mode 2).
 int run_clip_preprocess(cb_ctx* ctx, const cb_surface_pool* pool, const int32_t* slots, int n, int res, int out_mode, int layout_patch,
                         int k_pad, int dtype, const float mean[3], const float std_[3], void* out, cudaStream_t stream) {
   int rc = check_pool(ctx, pool, n, slots);
@@ -793,101 +757,140 @@ int run_clip_preprocess(cb_ctx* ctx, const cb_surface_pool* pool, const int32_t*
   int max_slot = 0;
   for (int i = 0; i < n; ++i) max_slot = std::max(max_slot, (int)slots[i]);
 
-  const char* kernel = getenv("CB_PRE_KERNEL");
-  if (!kernel || strcmp(kernel, "simt") != 0) {
-    rc = run_clip_preprocess_tc(ctx, pool, d_slots, n, max_slot, res, out_mode, layout_patch, k_pad, dtype, tx, ty, out, stream);
-    if (rc <= 0) return rc;  // ran, or failed; 1 = not served by the tensor-pipe kernel
+  uint8_t* u8 = (uint8_t*)out;
+  if (out_mode != 0) {
+    const size_t u8_bytes = (size_t)n * 3 * res * res;
+    if (ctx->tmp_u8_cap < u8_bytes) {
+      if (ctx->d_tmp_u8) {
+        CB_CUDA(ctx, cudaStreamSynchronize(stream));  // a previous call's pack kernel may still read the old buffer
+        cudaFree(ctx->d_tmp_u8);
+      }
+      ctx->tmp_u8_cap = std::max(u8_bytes, (size_t)64 << 20);
+      CB_CUDA(ctx, cudaMalloc(&ctx->d_tmp_u8, ctx->tmp_u8_cap));
+    }
+    u8 = ctx->d_tmp_u8;
   }
-  return run_clip_preprocess_simt(ctx, pool, d_slots, n, max_slot, res, out_mode, layout_patch, k_pad, dtype, tx, ty, out, stream);
+
+  const char* kernel = getenv("CB_PRE_KERNEL");
+  rc = 1;
+  if (!kernel || strcmp(kernel, "simt") != 0) rc = run_clip_preprocess_tc(ctx, pool, d_slots, n, max_slot, res, tx, ty, u8, stream);
+  if (rc == 1) rc = run_clip_preprocess_simt(ctx, pool, d_slots, n, max_slot, res, tx, ty, u8, stream);  // not served by the tensor pipe
+  if (rc || out_mode == 0) return rc;
+  const PackArgs q{u8, ctx->d_norm_lut, n, res, dtype, layout_patch, k_pad, out};
+  mark_launch(ctx, CB_PROF_PREPROCESS, stream);
+  if (out_mode == 1) {
+    const size_t total = (size_t)n * 3 * res * res;
+    normalize_pack_kernel<<<(unsigned)((total + 255) / 256), 256, 0, stream>>>(q);
+  } else {
+    const int kz = (3 * layout_patch * layout_patch + 7) & ~7;  // pack_patches_kernel's table: at most 12 KB whatever k_pad is
+    pack_patches_kernel<<<dim3(res / layout_patch, n), 256, kz * sizeof(int), stream>>>(q);
+  }
+  CB_CUDA(ctx, cudaGetLastError());
+  return CB_OK;
+}
+
+// The prologue the per-pixel surface kernels share: checks the pool, the slot list and the output, describes the pool in `s` and
+// uploads the slot list.  Returns 1 when there is nothing to launch (n == 0).
+static int open_pool(cb_ctx* ctx, const cb_surface_pool* pool, const int32_t* slots, int n, const void* out, Surface* s, cudaStream_t stream) {
+  int rc = check_pool(ctx, pool, n, slots);
+  if (rc) return rc;
+  if (n == 0) return 1;
+  if (!out) return fail(ctx, CB_ERR_ARG, "null output");
+  *s = Surface{(const uint8_t*)pool->base, pool->slot_stride, nullptr, pool->width, pool->height, pool->pitch, pool->luma_rows, pool->format};
+  return upload_slots(ctx, slots, n, stream, &s->slots);
 }
 
 static int run_simple(cb_ctx* ctx, const cb_surface_pool* pool, const int32_t* slots, int n, int out_w, int out_h, uint8_t* out, bool bilinear,
                       cudaStream_t stream) {
-  int rc = check_pool(ctx, pool, n, slots);
-  if (rc) return rc;
-  if (n == 0) return CB_OK;
-  if (!out) return fail(ctx, CB_ERR_ARG, "null output");
-  if (!is_nv12(pool->format)) return fail(ctx, CB_ERR_UNSUPPORTED, "NV12 surfaces only");
   SimpleArgs a{};
-  a.base = (const uint8_t*)pool->base, a.slot_stride = pool->slot_stride;
-  a.n = n, a.w = pool->width, a.h = pool->height, a.pitch = pool->pitch, a.luma_rows = pool->luma_rows;
-  a.out_w = out_w, a.out_h = out_h, a.out = out, a.format = pool->format;
-  rc = upload_slots(ctx, slots, n, stream, &a.slots);
-  if (rc) return rc;
+  int rc = open_pool(ctx, pool, slots, n, out, &a.s, stream);
+  if (rc) return rc > 0 ? CB_OK : rc;
+  if (!is_nv12(pool->format)) return fail(ctx, CB_ERR_UNSUPPORTED, "NV12 surfaces only");
   if (bilinear && (out_w <= 0 || out_h <= 0)) return fail(ctx, CB_ERR_ARG, "bad output size");
+  a.n = n, a.out_w = out_w, a.out_h = out_h, a.out = out;
   mark_launch(ctx, CB_PROF_PREPROCESS, stream);
   if (bilinear) {
     const long long total = (long long)n * out_w * out_h;
     bilinear_u8_kernel<<<(unsigned)((total + 255) / 256), 256, 0, stream>>>(a);
   } else {
-    const long long total = (long long)n * a.h * ((a.w + 1) / 2);
+    const long long total = (long long)n * a.s.h * ((a.s.w + 1) / 2);
     nv12_to_rgb_kernel<<<(unsigned)((total + 255) / 256), 256, 0, stream>>>(a);
   }
   CB_CUDA(ctx, cudaGetLastError());
   return CB_OK;
 }
 
-// OpenCV resize(): fx = float((dx + 0.5) * scale - 0.5) with scale = 1 / (dst / src) in double; interpolateCubic in float.
-static const CubicTaps* get_cubic_taps(cb_ctx* ctx, int src, int dst) {
+// cv2.resize() tap tables for one axis (resize.cpp): fx = float((dx + 0.5) * scale - 0.5) with scale = 1 / (dst / src) in double,
+// weights quantised to 2^11.  Cubic: interpolateCubic in float, 4 taps from sx - 1.  Linear: 2 taps from sx; the column table zeroes
+// fx at the borders, the row table clamps rows instead.
+enum TapKind { kTapsCubic, kTapsLinearZeroBorder, kTapsLinearClamp };
+
+static const ResizeTaps* get_resize_taps(cb_ctx* ctx, int src, int dst, TapKind kind) {
   std::lock_guard<std::mutex> lk(ctx->mu);
-  auto key = std::make_pair(src, dst);
-  auto it = ctx->cubic_taps.find(key);
-  if (it != ctx->cubic_taps.end()) return &it->second;
+  const auto key = std::make_tuple(src, dst, (int)kind);
+  auto it = ctx->resize_taps.find(key);
+  if (it != ctx->resize_taps.end()) return &it->second;
+  const int nt = kind == kTapsCubic ? 4 : 2;
   std::vector<int> first(dst);
-  std::vector<short> wq(4 * (size_t)dst);
-  std::vector<double> wf(4 * (size_t)dst);
+  std::vector<short> wq(nt * (size_t)dst);
+  std::vector<double> wf(kind == kTapsCubic ? 4 * (size_t)dst : 0);
   const double inv_scale = (double)dst / (double)src, scale = 1.0 / inv_scale;
   for (int d = 0; d < dst; ++d) {
     float fx = (float)((d + 0.5) * scale - 0.5);
-    const int sx = (int)std::floor(fx);
+    int sx = (int)std::floor(fx);
     fx -= (float)sx;
-    first[d] = sx - 1;
-    const float A = -0.75f;
     float c[4];
-    c[0] = ((A * (fx + 1.f) - 5.f * A) * (fx + 1.f) + 8.f * A) * (fx + 1.f) - 4.f * A;
-    c[1] = ((A + 2.f) * fx - (A + 3.f)) * fx * fx + 1.f;
-    c[2] = ((A + 2.f) * (1.f - fx) - (A + 3.f)) * (1.f - fx) * (1.f - fx) + 1.f;
-    c[3] = 1.f - c[0] - c[1] - c[2];
-    // float path: the same Keys kernel evaluated in double at the double-precision phase (what a correctly rounded result needs)
-    const double pos = (d + 0.5) * scale - 0.5, fr = pos - std::floor(pos), Ad = -0.75;
-    const double cd[4] = {((Ad * (fr + 1) - 5 * Ad) * (fr + 1) + 8 * Ad) * (fr + 1) - 4 * Ad, ((Ad + 2) * fr - (Ad + 3)) * fr * fr + 1,
-                          ((Ad + 2) * (1 - fr) - (Ad + 3)) * (1 - fr) * (1 - fr) + 1, 0.0};
-    for (int k = 0; k < 4; ++k) {
+    if (kind == kTapsCubic) {
+      first[d] = sx - 1;
+      const float A = -0.75f;
+      c[0] = ((A * (fx + 1.f) - 5.f * A) * (fx + 1.f) + 8.f * A) * (fx + 1.f) - 4.f * A;
+      c[1] = ((A + 2.f) * fx - (A + 3.f)) * fx * fx + 1.f;
+      c[2] = ((A + 2.f) * (1.f - fx) - (A + 3.f)) * (1.f - fx) * (1.f - fx) + 1.f;
+      c[3] = 1.f - c[0] - c[1] - c[2];
+      // float path: the same Keys kernel evaluated in double at the double-precision phase (what a correctly rounded result needs)
+      const double pos = (d + 0.5) * scale - 0.5, fr = pos - std::floor(pos), Ad = -0.75;
+      double* w = &wf[4 * (size_t)d];
+      w[0] = ((Ad * (fr + 1) - 5 * Ad) * (fr + 1) + 8 * Ad) * (fr + 1) - 4 * Ad;
+      w[1] = ((Ad + 2) * fr - (Ad + 3)) * fr * fr + 1;
+      w[2] = ((Ad + 2) * (1 - fr) - (Ad + 3)) * (1 - fr) * (1 - fr) + 1;
+      w[3] = 1.0 - w[0] - w[1] - w[2];
+    } else {
+      if (kind == kTapsLinearZeroBorder) {
+        if (sx < 0) fx = 0.f, sx = 0;
+        if (sx >= src - 1) fx = 0.f, sx = src - 1;
+      }
+      first[d] = sx;
+      c[0] = 1.f - fx, c[1] = fx;
+    }
+    for (int k = 0; k < nt; ++k) {
       const float q = std::nearbyint(c[k] * 2048.f);  // saturate_cast<short>(float) = cvRound: half to even
-      wq[4 * (size_t)d + k] = (short)std::min(32767.f, std::max(-32768.f, q));
-      wf[4 * (size_t)d + k] = k < 3 ? cd[k] : 1.0 - cd[0] - cd[1] - cd[2];
+      wq[nt * (size_t)d + k] = (short)std::min(32767.f, std::max(-32768.f, q));
     }
   }
-  CubicTaps t;
-  if (cudaMalloc(&t.d_first, dst * sizeof(int)) != cudaSuccess || cudaMalloc(&t.d_wq, 4 * (size_t)dst * sizeof(short)) != cudaSuccess ||
-      cudaMalloc(&t.d_wf, 4 * (size_t)dst * sizeof(double)) != cudaSuccess)
+  ResizeTaps t;
+  if (cudaMalloc(&t.d_first, dst * sizeof(int)) != cudaSuccess || cudaMalloc(&t.d_wq, wq.size() * sizeof(short)) != cudaSuccess ||
+      (!wf.empty() && cudaMalloc(&t.d_wf, wf.size() * sizeof(double)) != cudaSuccess))
     return nullptr;
   cudaMemcpy(t.d_first, first.data(), dst * sizeof(int), cudaMemcpyHostToDevice);
-  cudaMemcpy(t.d_wq, wq.data(), 4 * (size_t)dst * sizeof(short), cudaMemcpyHostToDevice);
-  cudaMemcpy(t.d_wf, wf.data(), 4 * (size_t)dst * sizeof(double), cudaMemcpyHostToDevice);
-  return &(ctx->cubic_taps[key] = t);
+  cudaMemcpy(t.d_wq, wq.data(), wq.size() * sizeof(short), cudaMemcpyHostToDevice);
+  if (!wf.empty()) cudaMemcpy(t.d_wf, wf.data(), wf.size() * sizeof(double), cudaMemcpyHostToDevice);
+  return &(ctx->resize_taps[key] = t);
 }
 
 static int run_resize_cubic(cb_ctx* ctx, const cb_surface_pool* pool, const int32_t* slots, int n, int out_w, int out_h, int mode, uint8_t* out,
                             cudaStream_t stream) {
-  int rc = check_pool(ctx, pool, n, slots);
-  if (rc) return rc;
-  if (n == 0) return CB_OK;
-  if (!out) return fail(ctx, CB_ERR_ARG, "null output");
+  CubicArgs a{};
+  int rc = open_pool(ctx, pool, slots, n, out, &a.s, stream);
+  if (rc) return rc > 0 ? CB_OK : rc;
   if (out_w <= 0 || out_h <= 0 || out_w > 8192 || out_h > 8192) return fail(ctx, CB_ERR_ARG, "bad output size %dx%d", out_w, out_h);
   if (mode != CB_CUBIC_OPENCV && mode != CB_CUBIC_IPP) return fail(ctx, CB_ERR_ARG, "unknown cubic mode %d", mode);
   if (is_nv12(pool->format) && ((pool->width | pool->height) & 1)) return fail(ctx, CB_ERR_UNSUPPORTED, "NV12 needs even dimensions");
-  const CubicTaps* tx = get_cubic_taps(ctx, pool->width, out_w);
-  const CubicTaps* ty = get_cubic_taps(ctx, pool->height, out_h);
+  const ResizeTaps* tx = get_resize_taps(ctx, pool->width, out_w, kTapsCubic);
+  const ResizeTaps* ty = get_resize_taps(ctx, pool->height, out_h, kTapsCubic);
   if (!tx || !ty) return fail(ctx, CB_ERR_CUDA, "cubic tap table allocation failed");
-  CubicArgs a{};
-  a.base = (const uint8_t*)pool->base, a.slot_stride = pool->slot_stride;
-  a.n = n, a.w = pool->width, a.h = pool->height, a.pitch = pool->pitch, a.luma_rows = pool->luma_rows, a.format = pool->format;
-  a.out_w = out_w, a.out_h = out_h, a.mode = mode, a.out = out;
+  a.n = n, a.out_w = out_w, a.out_h = out_h, a.mode = mode, a.out = out;
   a.n_vec = (out_w * 3) / 8 * 8;  // elements of a row handled by the 8-lane vector body of VResizeCubicVec_32s8u
   a.x0 = tx->d_first, a.wxq = tx->d_wq, a.wxf = tx->d_wf, a.y0 = ty->d_first, a.wyq = ty->d_wq, a.wyf = ty->d_wf;
-  rc = upload_slots(ctx, slots, n, stream, &a.slots);
-  if (rc) return rc;
   mark_launch(ctx, CB_PROF_PREPROCESS, stream);
   const long long total = (long long)n * out_w * out_h;
   resize_cubic_kernel<<<(unsigned)((total + 127) / 128), 128, 0, stream>>>(a);
@@ -895,66 +898,28 @@ static int run_resize_cubic(cb_ctx* ctx, const cb_surface_pool* pool, const int3
   return CB_OK;
 }
 
-// OpenCV resize() linear taps: the column table zeroes fx at the borders, the row table clamps rows instead (resize.cpp).
-static const CubicTaps* get_linear_taps(cb_ctx* ctx, int src, int dst, bool zero_at_border) {
-  std::lock_guard<std::mutex> lk(ctx->mu);
-  auto key = std::make_tuple(src, dst, zero_at_border ? 1 : 0);
-  auto it = ctx->linear_taps.find(key);
-  if (it != ctx->linear_taps.end()) return &it->second;
-  std::vector<int> first(dst);
-  std::vector<short> wq(2 * (size_t)dst);
-  const double inv_scale = (double)dst / (double)src, scale = 1.0 / inv_scale;
-  for (int d = 0; d < dst; ++d) {
-    float fx = (float)((d + 0.5) * scale - 0.5);
-    int sx = (int)std::floor(fx);
-    fx -= (float)sx;
-    if (zero_at_border) {
-      if (sx < 0) fx = 0.f, sx = 0;
-      if (sx >= src - 1) fx = 0.f, sx = src - 1;
-    }
-    first[d] = sx;
-    const float c[2] = {1.f - fx, fx};
-    for (int k = 0; k < 2; ++k) {
-      const float q = std::nearbyint(c[k] * 2048.f);  // saturate_cast<short>(float) = cvRound: half to even
-      wq[2 * (size_t)d + k] = (short)std::min(32767.f, std::max(-32768.f, q));
-    }
-  }
-  CubicTaps t;
-  if (cudaMalloc(&t.d_first, dst * sizeof(int)) != cudaSuccess || cudaMalloc(&t.d_wq, 2 * (size_t)dst * sizeof(short)) != cudaSuccess)
-    return nullptr;
-  cudaMemcpy(t.d_first, first.data(), dst * sizeof(int), cudaMemcpyHostToDevice);
-  cudaMemcpy(t.d_wq, wq.data(), 2 * (size_t)dst * sizeof(short), cudaMemcpyHostToDevice);
-  return &(ctx->linear_taps[key] = t);
-}
-
 static int run_video_tube(cb_ctx* ctx, const cb_surface_pool* pool, const int32_t* slots, int n, int out_w, int out_h, const float mean[3],
                           const float std_[3], float* out_f32, uint8_t* out_u8, cudaStream_t stream) {
-  int rc = check_pool(ctx, pool, n, slots);
-  if (rc) return rc;
-  if (n == 0) return CB_OK;
-  if (!out_f32 && !out_u8) return fail(ctx, CB_ERR_ARG, "null output");
+  TubeArgs a{};
+  int rc = open_pool(ctx, pool, slots, n, out_f32 ? (const void*)out_f32 : out_u8, &a.s, stream);
+  if (rc) return rc > 0 ? CB_OK : rc;
   if (out_w <= 0 || out_h <= 0 || out_w > 8192 || out_h > 8192) return fail(ctx, CB_ERR_ARG, "bad output size %dx%d", out_w, out_h);
   if (out_f32 && (!mean || !std_)) return fail(ctx, CB_ERR_ARG, "null mean/std");
   if (is_nv12(pool->format) && ((pool->width | pool->height) & 1)) return fail(ctx, CB_ERR_UNSUPPORTED, "NV12 needs even dimensions");
   if ((long long)n * out_w * out_h > 0x7fffffffLL) return fail(ctx, CB_ERR_ARG, "too many output pixels for one call");
-  TubeArgs a{};
-  a.base = (const uint8_t*)pool->base, a.slot_stride = pool->slot_stride;
-  a.n = n, a.w = pool->width, a.h = pool->height, a.pitch = pool->pitch, a.luma_rows = pool->luma_rows, a.format = pool->format;
-  a.out_w = out_w, a.out_h = out_h, a.out_f32 = out_f32, a.out_u8 = out_u8;
+  a.n = n, a.out_w = out_w, a.out_h = out_h, a.out_f32 = out_f32, a.out_u8 = out_u8;
   for (int c = 0; c < 3; ++c) a.mean[c] = mean ? mean[c] : 0.f, a.std_[c] = std_ ? std_[c] : 1.f;
-  if (a.w == out_w && a.h == out_h) {
+  if (a.s.w == out_w && a.s.h == out_h) {
     a.mode = 2;
-  } else if (a.w == 2 * out_w && a.h == 2 * out_h) {
+  } else if (a.s.w == 2 * out_w && a.s.h == 2 * out_h) {
     a.mode = 1;
   } else {
     a.mode = 0;
-    const CubicTaps* tx = get_linear_taps(ctx, a.w, out_w, true);
-    const CubicTaps* ty = get_linear_taps(ctx, a.h, out_h, false);
+    const ResizeTaps* tx = get_resize_taps(ctx, a.s.w, out_w, kTapsLinearZeroBorder);
+    const ResizeTaps* ty = get_resize_taps(ctx, a.s.h, out_h, kTapsLinearClamp);
     if (!tx || !ty) return fail(ctx, CB_ERR_CUDA, "linear tap table allocation failed");
     a.x0 = tx->d_first, a.ax = tx->d_wq, a.y0 = ty->d_first, a.by = ty->d_wq;
   }
-  rc = upload_slots(ctx, slots, n, stream, &a.slots);
-  if (rc) return rc;
   mark_launch(ctx, CB_PROF_PREPROCESS, stream);
   const long long total = (long long)n * out_w * out_h;
   video_tube_kernel<<<(unsigned)((total + 255) / 256), 256, 0, stream>>>(a);
@@ -965,8 +930,8 @@ static int run_video_tube(cb_ctx* ctx, const cb_surface_pool* pool, const int32_
 int bilinear_from_surface(cb_ctx* ctx, const void* base, int pitch, int luma_rows, int w, int h, int out_w, int out_h, uint8_t* out,
                           cudaStream_t stream) {
   SimpleArgs a{};
-  a.base = (const uint8_t*)base, a.slot_stride = 0, a.slots = nullptr;
-  a.n = 1, a.w = w, a.h = h, a.pitch = pitch, a.luma_rows = luma_rows, a.out_w = out_w, a.out_h = out_h, a.out = out, a.format = CB_FMT_NV12;
+  a.s = Surface{(const uint8_t*)base, 0, nullptr, w, h, pitch, luma_rows, CB_FMT_NV12};
+  a.n = 1, a.out_w = out_w, a.out_h = out_h, a.out = out;
   mark_launch(ctx, CB_PROF_PREPROCESS, stream);
   bilinear_u8_kernel<<<(out_w * out_h + 255) / 256, 256, 0, stream>>>(a);
   CB_CUDA(ctx, cudaGetLastError());

@@ -22,14 +22,15 @@
 //
 // A CTA owns (frame, 32 output columns) and walks the source rows top to bottom in units of 40 rows: TMA load of the NV12
 // window (Y + UV boxes) -> convert -> 14 MMAs -> epilogue -> vertical pass for the output rows that became complete.
-// ~105 KB of shared memory per CTA: two CTAs per SM overlap each other's phases.  Output: u8 [n][3][res][res]; normalisation +
-// patch packing is a second, bandwidth-trivial kernel (pack_patches_kernel / normalize_pack_kernel) so that this one stays small.
+// ~105 KB of shared memory per CTA: two CTAs per SM overlap each other's phases.  Output: u8 [n][3][res][res]; run_clip_preprocess
+// (preprocess.cu) normalises and packs it for both resample kernels.
 #include <algorithm>
 #include <cstring>
 #include <vector>
 
-#include <cuda_bf16.h>
+#include <cuda_fp16.h>
 
+#include "colour.cuh"
 #include "common.h"
 #include "ptx.cuh"
 
@@ -192,13 +193,8 @@ __global__ void __launch_bounds__(kTcThreads, 2)
         for (int h = 0; h < 2; ++h) {
           const int U = (int)((uv4 >> (16 * h)) & 0xff), V = (int)((uv4 >> (16 * h + 8)) & 0xff);
           int cr, cg, cb_;
-          if (sws) {
-            const int uu = (U << 3) - 1024, vv = (V << 3) - 1024;
-            cr = (vv * 13075) >> 16, cg = ((uu * -3209) >> 16) + ((vv * -6660) >> 16), cb_ = (uu * 16525) >> 16;
-          } else {
-            const int uo = U - 128, vo = V - 128;
-            cr = 1673527 * vo, cg = -852492 * vo - 409993 * uo, cb_ = 2116026 * uo;
-          }
+          if (sws) ColourSws::chroma(U, V, cr, cg, cb_);
+          else ColourOpenCv::chroma(U, V, cr, cg, cb_);
 #pragma unroll
           for (int rr = 0; rr < 2; ++rr) {
 #pragma unroll
@@ -206,12 +202,11 @@ __global__ void __launch_bounds__(kTcThreads, 2)
               const int Y = (int)((yw[rr] >> (16 * h + 8 * k)) & 0xff);
               int* o = px[rr][2 * h + k];
               if (sws) {
-                const int yv = (((Y << 3) - 128) * 9539) >> 16;
-                o[0] = __viaddmin_s32_relu(yv, cr, 255), o[1] = __viaddmin_s32_relu(yv, cg, 255), o[2] = __viaddmin_s32_relu(yv, cb_, 255);
+                const int yv = ColourSws::luma(Y);
+                o[0] = ColourSws::combine(yv, cr), o[1] = ColourSws::combine(yv, cg), o[2] = ColourSws::combine(yv, cb_);
               } else {
-                constexpr int kMax = (256 << 20) - 1;
-                const int yv = max(Y - 16, 0) * 1220542 + (1 << 19);
-                o[0] = __viaddmin_s32_relu(yv, cr, kMax) >> 20, o[1] = __viaddmin_s32_relu(yv, cg, kMax) >> 20, o[2] = __viaddmin_s32_relu(yv, cb_, kMax) >> 20;
+                const int yv = ColourOpenCv::luma(Y);
+                o[0] = ColourOpenCv::combine(yv, cr), o[1] = ColourOpenCv::combine(yv, cg), o[2] = ColourOpenCv::combine(yv, cb_);
               }
             }
           }
@@ -281,72 +276,6 @@ __global__ void __launch_bounds__(kTcThreads, 2)
   stage_taps(a.n_units - 1);
   __syncthreads();
   vertical(a.n_units - 1);
-}
-
-// u8 [n][3][res][res] -> normalised output: typed NCHW (mode 1) or zero-padded patch rows [n][(res/p)^2][k_pad] (mode 2)
-struct PackArgs {
-  const uint8_t* src;
-  const float* lut;  // [3][256]
-  int n, res, mode, dtype, patch, k_pad;
-  void* out;
-};
-
-__device__ __forceinline__ void store_out(void* out, size_t idx, float v, int dtype) {
-  if (dtype == CB_DT_F16) reinterpret_cast<__half*>(out)[idx] = __float2half_rn(v);
-  else if (dtype == CB_DT_BF16) reinterpret_cast<__nv_bfloat16*>(out)[idx] = __float2bfloat16_rn(v);
-  else reinterpret_cast<float*>(out)[idx] = v;
-}
-
-__global__ void normalize_pack_kernel(const PackArgs a) {  // mode 1: typed NCHW, one element per thread (parity-test output)
-  const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
-  const size_t plane = (size_t)a.res * a.res;
-  if (i >= 3 * plane * a.n) return;
-  const int ch = (int)((i / plane) % 3);
-  store_out(a.out, i, a.lut[ch * 256 + a.src[i]], a.dtype);
-}
-
-// mode 2: one CTA per (frame, patch row): the k -> (plane, y, x) map of a patch is built once in shared memory, then every thread
-// emits 8 consecutive elements of a zero-padded patch row per iteration as one 16-byte store.
-__global__ void __launch_bounds__(256) pack_patches_kernel(const PackArgs a) {
-  extern __shared__ int koff[];  // [k_pad]: (plane << 24) | offset inside the patch origin's plane, -1 = padding
-  const int g = a.res / a.patch, pp = a.patch * a.patch;
-  for (int k = threadIdx.x; k < a.k_pad; k += blockDim.x) {
-    int v = -1;
-    if (k < 3 * pp) {
-      const int ch = k / pp, yy = (k - ch * pp) / a.patch, xx = k - ch * pp - yy * a.patch;
-      v = (ch << 24) | (yy * a.res + xx);
-    }
-    koff[k] = v;
-  }
-  __syncthreads();
-  const int py = blockIdx.x, f = blockIdx.y;
-  const size_t plane = (size_t)a.res * a.res;
-  const uint8_t* img = a.src + (size_t)f * 3 * plane + (size_t)py * a.patch * a.res;
-  const int k8 = a.k_pad >> 3;
-  const bool bf = a.dtype == CB_DT_BF16;
-  for (int i = threadIdx.x; i < g * k8; i += blockDim.x) {
-    const int px = i / k8, kk = (i - px * k8) << 3;
-    uint32_t w[4];
-#pragma unroll
-    for (int e = 0; e < 4; ++e) {
-      float v[2];
-#pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        const int o = koff[kk + 2 * e + h];
-        const int ch = o >> 24;
-        v[h] = o < 0 ? 0.f : a.lut[ch * 256 + img[(size_t)ch * plane + (o & 0xFFFFFF) + px * a.patch]];
-      }
-      if (bf) {
-        __nv_bfloat162 b = __floats2bfloat162_rn(v[0], v[1]);
-        w[e] = *reinterpret_cast<uint32_t*>(&b);
-      } else {
-        __half2 hh = __floats2half2_rn(v[0], v[1]);
-        w[e] = *reinterpret_cast<uint32_t*>(&hh);
-      }
-    }
-    uint4* dst = reinterpret_cast<uint4*>(reinterpret_cast<uint16_t*>(a.out) + (((size_t)f * g + py) * g + px) * a.k_pad + kk);
-    *dst = make_uint4(w[0], w[1], w[2], w[3]);
-  }
 }
 
 // ------------------------------------------------------------------------------------------------ host
@@ -462,27 +391,15 @@ void release_tc_plans(cb_ctx* ctx) {
   plans(ctx).clear();
 }
 
-// Returns CB_OK when the tensor-pipe kernel ran; 1 when this configuration is not served by it (the caller falls back to the SIMT kernel).
-int run_clip_preprocess_tc(cb_ctx* ctx, const cb_surface_pool* pool, const int* d_slots, int n, int max_slot, int res, int out_mode, int patch, int k_pad,
-                           int dtype, const TapTable* tx, const TapTable* ty, void* out, cudaStream_t stream) {
+// Resamples into u8 `out` [n][3][res][res].  Returns CB_OK when the tensor-pipe kernel ran; 1 when this configuration is not served
+// by it (the caller falls back to the SIMT kernel).
+int run_clip_preprocess_tc(cb_ctx* ctx, const cb_surface_pool* pool, const int* d_slots, int n, int max_slot, int res, const TapTable* tx,
+                           const TapTable* ty, uint8_t* out, cudaStream_t stream) {
   if (pool->format != CB_FMT_NV12 && pool->format != CB_FMT_NV12_SWS) return 1;
   if (ty->max_taps > 40) return 1;
   const TcPlan* p = get_plan(ctx, tx, ty, res);
   if (!p) return fail(ctx, CB_ERR_CUDA, "preprocess plan allocation failed");
   if (!p->ok) return 1;
-  uint8_t* u8 = (uint8_t*)out;
-  const size_t u8_bytes = (size_t)n * 3 * res * res;
-  if (out_mode != 0) {
-    if (ctx->tmp_u8_cap < u8_bytes) {
-      if (ctx->d_tmp_u8) {
-        CB_CUDA(ctx, cudaStreamSynchronize(stream));
-        cudaFree(ctx->d_tmp_u8);
-      }
-      ctx->tmp_u8_cap = std::max(u8_bytes, (size_t)64 << 20);
-      CB_CUDA(ctx, cudaMalloc(&ctx->d_tmp_u8, ctx->tmp_u8_cap));
-    }
-    u8 = ctx->d_tmp_u8;
-  }
   const int W = pool->width, H = pool->height;
   CUtensorMap map_y, map_uv;
   uint64_t dims[3] = {(uint64_t)W, (uint64_t)H, (uint64_t)max_slot + 1};
@@ -500,26 +417,13 @@ int run_clip_preprocess_tc(cb_ctx* ctx, const cb_surface_pool* pool, const int* 
   a.slots = d_slots, a.n = n, a.res = res, a.ru = p->ru, a.n_units = p->n_units, a.y_begin = p->y_begin, a.kw = p->kw, a.kb = p->kb;
   a.colour = pool->format;
   a.x_lo = p->d_x_lo, a.tile_k0 = p->d_k0, a.tile_nk = p->d_nk, a.wtiles = p->d_w;
-  a.ymin = ty->d_min, a.ysize = ty->d_size, a.unit_last = p->d_unit_last, a.wy = ty->d_w, a.ty = ty->max_taps, a.out = u8;
+  a.ymin = ty->d_min, a.ysize = ty->d_size, a.unit_last = p->d_unit_last, a.wy = ty->d_w, a.ty = ty->max_taps, a.out = out;
   const int b_tile = (p->kb / 64) * 4096;
   const size_t smem = 1024 + (size_t)p->kw * 256 + 2 * (size_t)b_tile + ((((size_t)(p->ru + p->ru / 2) * p->kw) + 127) & ~(size_t)127) + (kRingRows * kRingStride + kVRows * kVTaps + 2 * kVRows + kMaxUnits) * 4 + 64;
   CB_CUDA(ctx, cudaFuncSetAttribute(clip_preprocess_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   mark_launch(ctx, CB_PROF_PREPROCESS, stream);
   clip_preprocess_tc_kernel<<<dim3(p->n_slabs, n), kTcThreads, smem, stream>>>(map_y, map_uv, a);
   CB_CUDA(ctx, cudaGetLastError());
-  if (out_mode != 0) {
-    PackArgs q{};
-    q.src = u8, q.lut = ctx->d_norm_lut, q.n = n, q.res = res, q.mode = out_mode, q.dtype = dtype, q.patch = patch, q.k_pad = k_pad, q.out = out;
-    mark_launch(ctx, CB_PROF_PREPROCESS, stream);
-    if (out_mode == 1) {
-      const size_t total = (size_t)n * 3 * res * res;
-      normalize_pack_kernel<<<(unsigned)((total + 255) / 256), 256, 0, stream>>>(q);
-    } else {
-      const int g = res / patch;
-      pack_patches_kernel<<<dim3(g, n), 256, k_pad * sizeof(int), stream>>>(q);
-    }
-    CB_CUDA(ctx, cudaGetLastError());
-  }
   return CB_OK;
 }
 

@@ -91,9 +91,10 @@ typedef struct cb_surface_pool {
 #define CB_LAYOUT_NCHW 0  /* out[n][3][res][res]                                   (reference tensor layout) */
 #define CB_LAYOUT_PATCH 1 /* out[n][(res/patch)^2][k_pad], k = (c, py, px), zero padded (tower input) */
 
-/* Fused colour-convert + resize + crop + normalise + pack.  Replaces, in one pass over the source
- * frame, cvcuda.cvtcolor_into (nvcodec_utils.py:178) and the reference CLIP transform chain
- * Resize(res, bicubic, antialias) -> CenterCrop(res) -> /255 -> Normalize (clip.py:48-62).
+/* Colour-convert + resize + crop + normalise + pack.  Replaces cvcuda.cvtcolor_into (nvcodec_utils.py:178)
+ * and the reference CLIP transform chain Resize(res, bicubic, antialias) -> CenterCrop(res) -> /255 ->
+ * Normalize (clip.py:48-62) with one pass over the source frame (colour, resize, crop -> u8 image) and
+ * one pass over the u8 image (normalise, pack).
  * slots[n] (host) selects the frames of `pool`; `out` is device memory of the chosen layout/dtype. */
 int cb_preprocess_clip(cb_ctx* ctx, const cb_surface_pool* pool, const int32_t* slots, int n, int res, int layout, int patch,
                        int k_pad, int dtype, const float mean[3], const float std_[3], void* out, void* stream);

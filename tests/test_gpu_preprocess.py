@@ -173,45 +173,48 @@ def test_resize_cubic_from_nv12_and_into_the_tower(ctx):
 # ------------------------------------------------------------------------------------ tensor-pipe kernel vs SIMT kernel
 @pytest.mark.parametrize(("h", "w", "pitch", "res", "colour"), [(1080, 1920, 2048, 224, "opencv"), (1080, 1920, 2048, 224, "swscale"), (2160, 3840, 3840, 384, "swscale"),
                                                                 (480, 854, 1024, 224, "swscale"), (720, 1280, 1280, 384, "opencv"), (360, 640, 640, 224, "opencv"),
-                                                                (2160, 3840, 3840, 224, "swscale"), (2160, 3840, 3840, 192, "opencv")])
+                                                                (2160, 3840, 3840, 224, "swscale"), (2160, 3840, 3840, 192, "opencv"), (1080, 1920, 0, 224, "rgb")])
 def test_tensor_pipe_preprocess_agrees_with_simt_kernel_and_oracle(ctx, monkeypatch, h, w, pitch, res, colour):
     """clip_preprocess_tc_kernel (horizontal pass as a banded fp16 hi/lo GEMM on wgmma, the default) against the SIMT kernel
     (CB_PRE_KERNEL=simt) and the oracle: same u8 image within the fp32-summation-order budget, both colour conversions, 1080p -> 224
     (bench shape), 4K -> 384 (SoViT shape, 24 vertical taps, 256-column windows), widths that are not a multiple of the window.
-    4K -> 192 has 45 vertical taps, more than the tensor-pipe kernel takes: there the default call falls back to the SIMT kernel."""
-    from gpu_helpers import nv12_pool
-
+    4K -> 192 has 45 vertical taps, more than the tensor-pipe kernel takes, and an RGB pool is never served by it: there the default
+    call runs the SIMT kernel too.  Both kernels share the normalise/pack step, so typed and patch outputs are exactly LUT(u8) of
+    each kernel's own u8 image."""
     frames = [color.synthetic_nv12(h, w, seed=60 + s) for s in range(2)]
-    rows = h + h // 2
-    buf = np.zeros((2, rows, pitch), dtype=np.uint8)
-    for i, f in enumerate(frames):
-        buf[i, :, :w] = f
-    pool = ctx.nv12_pool(torch.from_numpy(buf).cuda(), w, h, h, colour=colour)
-    got_tc = ctx.preprocess_clip_u8(pool, res=res).cpu().numpy()
-    from cosmos_curate_b200._lib import CurateB200Error
-
-    monkeypatch.setenv("CB_PRE_KERNEL", "simt")
-    try:
-        got_simt = ctx.preprocess_clip_u8(pool, res=res).cpu().numpy()
-    except CurateB200Error:  # a downscale beyond the SIMT kernel's (halved) tile window
-        assert (h, res) == (2160, 224)
-        got_simt = None
-    monkeypatch.delenv("CB_PRE_KERNEL")
     conv = color.nv12_to_rgb_swscale if colour == "swscale" else color.nv12_to_rgb
     rgb = np.stack([conv(f, h, w) for f in frames])
+    if colour == "rgb":
+        pool = ctx.rgb_pool(torch.from_numpy(rgb).cuda())
+    else:
+        buf = np.zeros((2, h + h // 2, pitch), dtype=np.uint8)
+        for i, f in enumerate(frames):
+            buf[i, :, :w] = f
+        pool = ctx.nv12_pool(torch.from_numpy(buf).cuda(), w, h, h, colour=colour)
+    lut = preprocess.normalize_lut()
+
+    def assert_typed_outputs_are_lut_of(u8):
+        want32 = np.stack([lut[c][u8[:, c]] for c in range(3)], axis=1)
+        np.testing.assert_array_equal(ctx.preprocess_clip(pool, res=res, dtype=torch.float32).cpu().numpy(), want32)
+        for patch, k_pad in ((14, 640), (16, 768)):
+            gp = ctx.preprocess_clip(pool, res=res, dtype=torch.float16, layout="patch", patch=patch, k_pad=k_pad).cpu().numpy()
+            np.testing.assert_array_equal(gp, preprocess.to_patches(want32.astype(np.float16), patch, k_pad))
+            gb = ctx.preprocess_clip(pool, res=res, dtype=torch.bfloat16, layout="patch", patch=patch, k_pad=k_pad).float().cpu().numpy()
+            want_bf = torch.from_numpy(want32).to(torch.bfloat16).float().numpy()
+            np.testing.assert_array_equal(gb, preprocess.to_patches(want_bf, patch, k_pad))
+
+    got_tc = ctx.preprocess_clip_u8(pool, res=res).cpu().numpy()
+    monkeypatch.setenv("CB_PRE_KERNEL", "simt")
+    got_simt = ctx.preprocess_clip_u8(pool, res=res).cpu().numpy()
+    assert_typed_outputs_are_lut_of(got_simt)
+    monkeypatch.delenv("CB_PRE_KERNEL")
     want = preprocess.clip_resize_crop_u8(rgb, res)
     _u8_budget(got_tc, want)
-    if got_simt is not None:
-        _u8_budget(got_simt, want)
-        _u8_budget(got_tc, got_simt, frac=2e-4)  # two fp32 summation orders apart
-    if res == 192:  # the default call ran the SIMT kernel too
+    _u8_budget(got_simt, want)
+    _u8_budget(got_tc, got_simt, frac=2e-4)  # two fp32 summation orders apart
+    if res == 192 or colour == "rgb":  # the default call ran the SIMT kernel too
         np.testing.assert_array_equal(got_tc, got_simt)
-    # typed + patch outputs of the default path are exactly LUT(u8)
-    lut = preprocess.normalize_lut()
-    want32 = np.stack([lut[c][got_tc[:, c]] for c in range(3)], axis=1)
-    np.testing.assert_array_equal(ctx.preprocess_clip(pool, res=res, dtype=torch.float32).cpu().numpy(), want32)
-    gp = ctx.preprocess_clip(pool, res=res, dtype=torch.float16, layout="patch", patch=14, k_pad=640).cpu().numpy()
-    np.testing.assert_array_equal(gp, preprocess.to_patches(want32.astype(np.float16), 14, 640))
+    assert_typed_outputs_are_lut_of(got_tc)
 
 
 def test_clip_preprocess_4k_rgb_frames_strong_downscale(ctx):
