@@ -39,7 +39,44 @@ def _stream_ptr(stream=None) -> int:
     return int(s.cuda_stream)
 
 
-class Context:
+# NV12 -> RGB arithmetic by name: "opencv" (CV-CUDA / cv2.cvtColor semantics, the reference's CUDA branch) or "swscale"
+# (libswscale's yuv420p -> rgb24, the reference's CPU decode branch)
+COLOURS = {"swscale": _lib.FMT_NV12_SWS, "opencv": _lib.FMT_NV12}
+
+
+def check_colour(colour: str) -> str:
+    """`colour` when it is a key of COLOURS, else ValueError (stages check it at construction, not at the first decode)."""
+    if colour not in COLOURS:
+        raise ValueError(f"colour={colour!r} not in {tuple(COLOURS)}")
+    return colour
+
+
+def even_size(width: int, height: int) -> tuple[int, int]:
+    """Surface size of a width x height stream: 4:2:0 chroma covers 2x2 pixels, so odd sizes round up."""
+    return (width + 1) & ~1, (height + 1) & ~1
+
+
+class _Handle:
+    """A library object behind `h`: `_destroy()` runs once, from close() or when the wrapper is collected."""
+
+    h = None
+
+    def _destroy(self) -> None:
+        raise NotImplementedError
+
+    def close(self):
+        if self.h:
+            self._destroy()
+            self.h = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:  # noqa: BLE001
+            pass
+
+
+class Context(_Handle):
     """One per process/GPU (cb_init).  Fails loudly when the library or a CUDA device is missing."""
 
     def __init__(self, device: int | None = None):
@@ -54,18 +91,10 @@ class Context:
         self.h = h
         self._children = weakref.WeakSet()  # towers / decoders created on this context: closed before it
 
-    def close(self):
-        if getattr(self, "h", None):
-            for child in list(self._children):
-                child.close()
-            self.lib.cb_destroy(self.h)
-            self.h = None
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:  # noqa: BLE001
-            pass
+    def _destroy(self):
+        for child in list(self._children):
+            child.close()
+        self.lib.cb_destroy(self.h)
 
     def launch_count(self) -> int:
         return int(self.lib.cb_launch_count(self.h))
@@ -88,13 +117,11 @@ class Context:
 
     # ---- surfaces -----------------------------------------------------------------------------
     def nv12_pool(self, buf: torch.Tensor, width: int, height: int, luma_rows: int | None = None, colour: str = "opencv") -> "Pool":
-        """buf: uint8 cuda [slots, rows, pitch] with rows >= luma_rows + height/2.  colour: "opencv" (CV-CUDA / cv2.cvtColor
-        semantics, the reference's CUDA branch) or "swscale" (libswscale's yuv420p -> rgb24, the reference's CPU decode branch)."""
+        """buf: uint8 cuda [slots, rows, pitch] with rows >= luma_rows + height/2.  colour: a key of COLOURS."""
         assert buf.is_cuda and buf.dtype == torch.uint8 and buf.dim() == 3 and buf.is_contiguous()
         luma_rows = height if luma_rows is None else luma_rows
         assert buf.shape[1] >= luma_rows + height // 2
-        fmt = {"opencv": _lib.FMT_NV12, "swscale": _lib.FMT_NV12_SWS}[colour]
-        return Pool(buf, SurfacePool(buf.data_ptr(), buf.shape[1] * buf.shape[2], width, height, buf.shape[2], luma_rows, fmt))
+        return Pool(buf, SurfacePool(buf.data_ptr(), buf.shape[1] * buf.shape[2], width, height, buf.shape[2], luma_rows, COLOURS[colour]))
 
     def rgb_pool(self, frames: torch.Tensor) -> "Pool":
         """frames: uint8 cuda [n, H, W, 3] (contiguous).  Rows are re-pitched to a 16-byte multiple if needed."""
@@ -228,7 +255,7 @@ class Pool:
         self.buf, self.desc = buf, desc  # keep the tensor alive while the descriptor is in use
 
 
-class VitTower:
+class VitTower(_Handle):
     """cb_vit_* wrapper: weights in (fp32 numpy, names of include/curate_b200.h cb_vit_set_tensor), embeddings / scores out."""
 
     def __init__(self, ctx: Context, cfg: dict, weights: dict, max_batch: int = 256, aesthetic: tuple | None = None):
@@ -255,16 +282,8 @@ class VitTower:
         self.k_pad = int(self.lib.cb_vit_k_pad(self.h))
         self.max_batch = max_batch
 
-    def close(self):
-        if getattr(self, "h", None):
-            self.lib.cb_vit_destroy(self.h)
-            self.h = None
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:  # noqa: BLE001
-            pass
+    def _destroy(self):
+        self.lib.cb_vit_destroy(self.h)
 
     def forward_patches(self, patches: torch.Tensor, want_features: bool = False):
         n = patches.shape[0]
@@ -288,7 +307,7 @@ class VitTower:
         return emb, feat, score
 
 
-class ShotNet:
+class ShotNet(_Handle):
     """cb_transnet_* wrapper: the reference state_dict in (its own key names), per-frame transition probabilities out."""
 
     UNUSED_KEYS = ("cls_layer2.weight", "cls_layer2.bias")  # many-hot head: built by the reference, never used by forward()
@@ -307,16 +326,8 @@ class ShotNet:
         check(self.lib.cb_transnet_finalize(self.h, max_windows), "cb_transnet_finalize", ctx.h)
         self.max_windows = max_windows
 
-    def close(self):
-        if getattr(self, "h", None):
-            self.lib.cb_transnet_destroy(self.h)
-            self.h = None
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:  # noqa: BLE001
-            pass
+    def _destroy(self):
+        self.lib.cb_transnet_destroy(self.h)
 
     def forward(self, windows: torch.Tensor) -> torch.Tensor:
         """uint8 cuda [B, T, 27, 48, 3] -> fp32 cuda [B, T, 1] (the reference model's call signature, transnetv2.py:569-580)."""
@@ -380,7 +391,7 @@ def nvdec_available(ctx: Context) -> bool:
     return _NVDEC_OK[ctx.device]
 
 
-class Decoder:
+class Decoder(_Handle):
     """One decode session: NVDEC (cb_decoder_*), or libavcodec on the host where the device's NVDEC is not usable (nvdec_available).
     Not thread-safe: use one per host thread."""
 
@@ -395,11 +406,9 @@ class Decoder:
         self.h = h
         ctx._children.add(self)
 
-    def close(self):
-        if getattr(self, "h", None):
-            if not self.host:
-                self.lib.cb_decoder_destroy(self.h)
-            self.h = None
+    def _destroy(self):
+        if not self.host:
+            self.lib.cb_decoder_destroy(self.h)
 
     def _host_decode(self, buf, ids, pool, slots, seek_keyframes: bool) -> dict:
         """decode() on the host: the same request checks and statistics as cb_decoder_decode_ex, pictures uploaded as NV12."""
@@ -407,7 +416,7 @@ class Decoder:
 
         idx = mp4_index(buf, self.ctx)  # CB_ERR_DEMUX on anything that is not an mp4 with a video track
         n = idx["n_samples"]
-        w2, h2 = (idx["width"] + 1) & ~1, (idx["height"] + 1) & ~1
+        w2, h2 = even_size(idx["width"], idx["height"])
         st = {"frames_decoded": 0, "frames_emitted": 0, "coded": ((idx["width"] + 15) & ~15, (idx["height"] + 15) & ~15), "size": (idx["width"], idx["height"])}
         if pool is not None and len(ids) == 0:
             return st
@@ -446,12 +455,6 @@ class Decoder:
             raise _lib.CurateB200Error(-4, "cb_decoder_decode", f"decode: {emitted} of {len(ids)} frames delivered")
         st["frames_emitted"] = emitted
         return st
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:  # noqa: BLE001
-            pass
 
     def decode(self, data, frame_ids, pool: Pool, dst_slots, seek_keyframes: bool = False) -> dict:
         """Decode `data` (mp4 bytes) and copy display-order frames `frame_ids` (ascending, repeats allowed)
@@ -525,7 +528,7 @@ def decode_thumbnails(dec: Decoder, data, out_w: int, out_h: int, n_frames: int)
 
 def alloc_nv12_pool(ctx: Context, slots: int, width: int, height: int, colour: str = "opencv") -> Pool:
     """Device NV12 surface pool for `slots` frames of width x height (pitch aligned to 256 bytes); `colour` as Context.nv12_pool."""
-    w2, h2 = (width + 1) & ~1, (height + 1) & ~1
+    w2, h2 = even_size(width, height)
     pitch = (w2 + 255) // 256 * 256
     buf = torch.empty((slots, h2 + h2 // 2, pitch), dtype=torch.uint8, device=f"cuda:{ctx.device}")
     return ctx.nv12_pool(buf, w2, h2, h2, colour)
@@ -562,35 +565,73 @@ def device_numa_cpus(ctx: Context) -> tuple[int | None, list[int]]:
         return None, []
 
 
-class SessionTable:
-    """One NVDEC session per stream shape for a single-threaded caller (the same rule DecoderPool applies per worker thread:
-    a session that is fed another resolution is destroyed and re-created by the driver, ~0.4 s each time)."""
+class ShapeCache:
+    """One object per stream shape (any hashable, normally (width, height)), made by `create(shape)` on first use.  At most
+    MAX_SHAPES are kept: a new shape beyond that hands the least recently used object to `close`."""
 
     MAX_SHAPES = 4
 
-    def __init__(self, ctx: Context):
-        self.ctx = ctx
-        self._decs: dict = {}
+    def __init__(self, create, close):
+        self._create, self._close = create, close
+        self._items: dict = {}  # least recently used first
 
-    def get(self, shape) -> Decoder:
-        d = self._decs.pop(shape, None)
-        if d is None or d.h is None:
-            while len(self._decs) >= self.MAX_SHAPES:
-                self._decs.pop(next(iter(self._decs))).close()  # least recently used
-            d = Decoder(self.ctx)
-        self._decs[shape] = d
-        return d
+    def get(self, shape):
+        v = self._items.pop(shape, None)
+        if v is None:
+            while len(self._items) >= self.MAX_SHAPES:
+                self._close(self._items.pop(next(iter(self._items))))
+            v = self._create(shape)
+        self._items[shape] = v
+        return v
+
+    def values(self) -> list:
+        return list(self._items.values())
 
     def close(self) -> None:
-        for d in self._decs.values():
-            d.close()
-        self._decs.clear()
+        for v in self._items.values():
+            self._close(v)
+        self._items.clear()
+
+
+class SessionTable(ShapeCache):
+    """One NVDEC session per stream shape for a single-threaded caller (DecoderPool keeps one table per worker thread): a
+    session that is fed another resolution is destroyed and re-created by the driver, ~0.4 s each time."""
+
+    def __init__(self, ctx: Context):
+        super().__init__(lambda shape: Decoder(ctx), Decoder.close)
+        self.ctx = ctx
+
+
+class SurfacePools:
+    """A stage's NV12 decode surfaces: per stream size (a ShapeCache) a ring of `depth` pools, so that decode into one pool
+    overlaps the kernels that read another.  A pool holds the smallest min_slots * 2^k slots that fit the request; a pool
+    that is too small is dropped before its replacement is allocated."""
+
+    def __init__(self, ctx: Context, depth: int, min_slots: int, colour: str):
+        self.ctx, self.min_slots, self.colour = ctx, min_slots, colour
+        self._rings = ShapeCache(lambda size: [None] * depth, list.clear)
+
+    def get(self, size: tuple[int, int], n: int, r: int = 0) -> Pool:
+        """Pool `r` of the ring for streams of `size` = (width, height), with at least `n` slots."""
+        ring = self._rings.get(size)
+        cap = self.min_slots
+        while cap < n:
+            cap *= 2
+        if ring[r] is None or ring[r].buf.shape[0] < cap:
+            ring[r] = None
+            ring[r] = alloc_nv12_pool(self.ctx, cap, size[0], size[1], self.colour)
+        return ring[r]
+
+    def clear(self) -> None:
+        self._rings.close()
 
 
 class DecoderPool:
-    """Persistent NVDEC sessions behind a thread pool: one `Decoder` per worker thread, created on first use and kept across
-    calls (session creation costs ~10 ms and a context-lock round trip), worker threads pinned to the host CPUs of the GPU's
-    NUMA node (bitstream parsing + H2D staging are host work: on a two-socket 8-GPU box the far socket costs decode rate)."""
+    """Persistent NVDEC sessions behind a thread pool: one `SessionTable` per worker thread, created on first use and kept
+    across calls (session creation costs ~10 ms and a context-lock round trip), worker threads pinned to the host CPUs of the
+    GPU's NUMA node (bitstream parsing + H2D staging are host work: on a two-socket 8-GPU box the far socket costs decode rate)."""
+
+    MAX_SHAPES = SessionTable.MAX_SHAPES  # sessions a worker thread keeps
 
     def __init__(self, ctx: Context, sessions: int, pin: bool = True):
         import threading
@@ -600,7 +641,7 @@ class DecoderPool:
         self.numa_node, cpus = device_numa_cpus(ctx) if pin else (None, [])
         self.cpus = cpus
         self._tls = threading.local()
-        self._decoders: list[Decoder] = []
+        self._tables: list[SessionTable] = []
         self._lock = threading.Lock()
         self._tp = ThreadPoolExecutor(max_workers=self.sessions, thread_name_prefix="cb-nvdec", initializer=self._init_thread)
 
@@ -613,37 +654,56 @@ class DecoderPool:
             except OSError:
                 pass
 
-    MAX_SHAPES = 4  # sessions a worker thread keeps, one per stream shape (least recently used closed beyond that)
-
     def decoder(self, shape=None) -> Decoder:
         """This thread's session for streams of `shape` (any hashable, normally (width, height)).  A cuvid decoder is bound to
         one coded size: feeding a session a clip of another resolution destroys and re-creates it (hundreds of ms, serialised
         in the driver - measured: a 720p / 1080p / 4K mix ran 4-12x below the NVDEC rate with one session per thread), so a
         thread keeps one session per shape instead."""
-        decs = getattr(self._tls, "decs", None)
-        if decs is None:
-            decs = self._tls.decs = {}
-        d = decs.pop(shape, None)
-        if d is None or d.h is None:
-            while len(decs) >= self.MAX_SHAPES:
-                old = decs.pop(next(iter(decs)))
-                with self._lock:
-                    if old in self._decoders:
-                        self._decoders.remove(old)
-                old.close()
-            d = Decoder(self.ctx)
+        table = getattr(self._tls, "table", None)
+        if table is None:
+            table = self._tls.table = SessionTable(self.ctx)
             with self._lock:
-                self._decoders.append(d)
-        decs[shape] = d  # most recently used last
-        return d
+                self._tables.append(table)
+        return table.get(shape)
+
+    @property
+    def _decoders(self) -> list[Decoder]:
+        """The open sessions of every worker thread."""
+        with self._lock:
+            return [d for t in self._tables for d in t.values()]
 
     def submit(self, fn, *args, shape=None, **kw):
         """fn(decoder, *args, **kw) on a pool thread with that thread's own session (for streams of `shape`, see decoder())."""
         return self._tp.submit(lambda: fn(self.decoder(shape), *args, **kw))
 
+    def submit_group(self, pool: Pool, shape, jobs, seek_keyframes: bool = False) -> list:
+        """Decode each (data, frame ids) job into `pool`, the jobs' frames in consecutive slots from slot 0, on sessions for
+        streams of `shape`.  -> [(first slot of the job, future of its Decoder.decode statistics)] in job order."""
+        def decode(dec, data, ids, slots):
+            return dec.decode(data, ids, pool, slots, seek_keyframes=seek_keyframes)
+
+        out, first = [], 0
+        for data, ids in jobs:
+            out.append((first, self.submit(decode, data, ids, np.arange(first, first + len(ids), dtype=np.int32), shape=shape)))
+            first += len(ids)
+        return out
+
     def close(self) -> None:
         self._tp.shutdown(wait=True)
         with self._lock:
-            for d in self._decoders:
-                d.close()
-            self._decoders.clear()
+            for t in self._tables:
+                t.close()
+            self._tables.clear()
+
+
+def collect_group(jobs) -> tuple[int, list]:
+    """Wait for the jobs of DecoderPool.submit_group -> (frames decoded by the jobs that succeeded, summed; per job its
+    CurateB200Error or None, in job order)."""
+    decoded, errs = 0, []
+    for _, fut in jobs:
+        try:
+            decoded += fut.result()["frames_decoded"]
+            errs.append(None)
+        except _lib.CurateB200Error as e:
+            errs.append(e)
+    return decoded, errs

@@ -18,7 +18,7 @@ from .. import _lib
 from .._lib import CurateB200Error
 from ..data_model import LazyData, StageTimer
 from ..interfaces import CuratorStage, CuratorStageResource
-from ..runtime import SessionTable, alloc_nv12_pool, decode_thumbnails, get_context, mp4_index
+from ..runtime import SessionTable, SurfacePools, check_colour, decode_thumbnails, get_context, mp4_index
 from ..sampling import FrameExtractionPolicy
 
 try:
@@ -55,10 +55,7 @@ class ClipFrameExtractionStage(CuratorStage):
         self._timer = StageTimer(self)
         # "swscale": RGB frames bit-identical to the reference stage's (PyAV frame.to_ndarray("rgb24") = libswscale's yuv420p
         # -> rgb24, decoder_utils.py:439-451); "opencv": CV-CUDA / cv2.cvtColor semantics (the reference's nvcodec_utils branch)
-        if colour not in ("swscale", "opencv"):
-            msg = f"colour={colour!r} not in ('swscale', 'opencv')"
-            raise ValueError(msg)
-        self._colour = colour
+        self._colour = check_colour(colour)
         self._extraction_policies = extraction_policies
         self._target_fps = [2] if target_fps is None else target_fps
         self._target_res = (-1, -1) if target_res is None else target_res
@@ -79,35 +76,19 @@ class ClipFrameExtractionStage(CuratorStage):
     def stage_setup(self) -> None:
         self._ctx = get_context()
         self._sessions = SessionTable(self._ctx)  # one NVDEC session per clip resolution (a mixed stream would re-create a single one per clip)
-        self._pools: dict[tuple, object] = {}
+        # one pool per resolution, at least 64 slots: a 64-slot 1080p pool is 0.2 GB and the actor may own only 0.25 GPU
+        self._pools = SurfacePools(self._ctx, 1, 64, self._colour)
 
     def destroy(self) -> None:
         if getattr(self, "_sessions", None):
             self._sessions.close()
-
-    MAX_POOLS = 4  # resolutions kept resident (LRU); a 64-slot 1080p pool is 0.2 GB and the actor may own only 0.25 GPU
-
-    def _surface_pool(self, width: int, height: int, n_frames: int):
-        """One pool per resolution, capacity a power of two >= 64 (grown by replacement), least recently used evicted."""
-        key = (width, height)
-        pool = self._pools.pop(key, None)
-        cap = 64
-        while cap < n_frames:
-            cap *= 2
-        if pool is None or pool.buf.shape[0] < cap:
-            pool = None  # drop the smaller pool before allocating its replacement
-            while len(self._pools) >= self.MAX_POOLS:
-                self._pools.pop(next(iter(self._pools)))
-            pool = alloc_nv12_pool(self._ctx, cap, width, height, self._colour)
-        self._pools[key] = pool  # most recently used last
-        return pool
 
     def _extract(self, data) -> dict[str, np.ndarray]:
         idx = mp4_index(data)
         ts = sampling.timestamps_from_index(idx["pts"], idx["timescale"])
         plan = sampling.plan_extraction(ts, self._extraction_policies, self._target_fps)
         all_ids = np.unique(np.concatenate(list(plan.values()))).astype(np.int32)
-        pool = self._surface_pool(idx["width"], idx["height"], len(all_ids))
+        pool = self._pools.get((idx["width"], idx["height"]), len(all_ids))
         self._sessions.get((idx["width"], idx["height"])).decode(data, all_ids, pool, np.arange(len(all_ids), dtype=np.int32))
         slots = np.arange(len(all_ids), dtype=np.int32)
         if self._target_res[0] > 0 and self._target_res[1] > 0:  # only 3 * th * tw bytes per frame cross PCIe (150 KB instead of 6 MB)

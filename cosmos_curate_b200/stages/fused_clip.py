@@ -29,7 +29,7 @@ from .._lib import CurateB200Error
 from ..data_model import StageTimer
 from ..interfaces import CuratorStage, CuratorStageResource, ModelInterface
 from ..models.clip_aesthetics import CLIPAestheticScorer
-from ..runtime import DecoderPool, alloc_nv12_pool, get_context, mp4_index
+from ..runtime import DecoderPool, SurfacePools, check_colour, collect_group, even_size, get_context, mp4_index
 
 try:
     from loguru import logger
@@ -78,10 +78,7 @@ class NvdecClipAestheticStage(CuratorStage):
         self._source = source
         # colour conversion of the decoded NV12 surfaces inside the fused kernel: "swscale" = bit-identical to the RGB frames the
         # reference's CPU decode hands to CLIP (libswscale yuv420p -> rgb24, decoder_utils.py:439-451), "opencv" = CV-CUDA semantics
-        if colour not in ("swscale", "opencv"):
-            error_msg = f"colour={colour!r} not in ('swscale', 'opencv')"
-            raise ValueError(error_msg)
-        self._colour = colour
+        self._colour = check_colour(colour)
         # clip_extraction_target_res of the reference pipeline (splitting_pipeline -> ClipFrameExtractionStage(target_res=(r, r))):
         # frames are squashed to (h, w) with cv2 INTER_CUBIC before the CLIP transforms (decoder_utils.py:666-670).  None / (-1, -1)
         # = native resolution into the antialiased short-side resize (the reference default).
@@ -94,7 +91,7 @@ class NvdecClipAestheticStage(CuratorStage):
         # SigLIPImageEmbeddings (score_threshold=None: nothing is filtered, clip.openai_embedding is the output).
         self._model = model if model is not None else CLIPAestheticScorer(max_batch=max_batch)
         self._reduce_fn = np.min
-        self._pools: dict[tuple[int, int], list] = {}
+        self._pools: SurfacePools | None = None
         self.last_call_stats: dict = {}
 
     @property
@@ -124,13 +121,15 @@ class NvdecClipAestheticStage(CuratorStage):
             error_msg = "embedding-only mode (score_threshold=None) needs write_embedding=True"
             raise ValueError(error_msg)
         self._decode_pool = DecoderPool(self._ctx, self._num_decoders)  # 7 NVDEC engines need ~20 sessions in flight (DESIGN.md 5)
+        self._pools = SurfacePools(self._ctx, self.RING, self._max_batch, self._colour)
         self._host: list[tuple[torch.Tensor, torch.Tensor | None]] = []
 
     def destroy(self) -> None:
         if getattr(self, "_decode_pool", None):
             self._decode_pool.close()
             self._decode_pool = None
-        self._pools.clear()
+        if self._pools is not None:
+            self._pools.clear()
 
     # ---- helpers ---------------------------------------------------------------------------------
     def _plan_span(self, clip, video):
@@ -148,7 +147,7 @@ class NvdecClipAestheticStage(CuratorStage):
                 cached = self._video_index[id(video)] = (data, idx, sampling.timestamps_from_index(idx["pts"], idx["timescale"]))
             _, idx, ts = cached
             ids = sampling.span_frame_ids(ts, clip.span, self._target_fps)
-            return data, ids, ((idx["width"] + 1) & ~1, (idx["height"] + 1) & ~1)
+            return data, ids, even_size(idx["width"], idx["height"])
         except (CurateB200Error, ValueError) as e:
             logger.error(f"Error extracting frames from clip {clip.uuid}: {e}")
             clip.errors["frame_extraction"] = "video_decode_failed"
@@ -169,7 +168,7 @@ class NvdecClipAestheticStage(CuratorStage):
             idx = mp4_index(data)
             ts = sampling.timestamps_from_index(idx["pts"], idx["timescale"])
             ids, counts = sampling.frame_ids(ts, sampling.FrameExtractionPolicy.sequence, self._target_fps)
-            return data, np.repeat(ids, counts).astype(np.int32), ((idx["width"] + 1) & ~1, (idx["height"] + 1) & ~1)
+            return data, np.repeat(ids, counts).astype(np.int32), even_size(idx["width"], idx["height"])
         except (CurateB200Error, ValueError) as e:
             self._decode_failed(clip, e)
             return None
@@ -183,19 +182,6 @@ class NvdecClipAestheticStage(CuratorStage):
 
     RING = 3  # surface pools per resolution: tower on batch k, NVDEC filling k+1 and k+2
 
-    def _pool(self, size, r: int):
-        ring = self._pools.get(size)
-        if ring is None:
-            if len(self._pools) >= 4:  # mixed-resolution runs: keep the four most recent resolutions (LRU), free the rest
-                self._pools.pop(next(iter(self._pools)))
-            ring = [None] * self.RING
-        else:
-            self._pools.pop(size)
-        self._pools[size] = ring  # most recently used last
-        if ring[r] is None:
-            ring[r] = alloc_nv12_pool(self._ctx, self._max_batch, size[0], size[1], self._colour)
-        return ring[r]
-
     def _host_buffers(self, r: int):
         while len(self._host) <= r:
             tower = self._model.tower
@@ -205,7 +191,7 @@ class NvdecClipAestheticStage(CuratorStage):
         return self._host[r]
 
     def _make_batches(self, by_size):
-        """[(size, [(clip, data, ids, first_slot)])]: whole clips, at most max_batch frames, one resolution per batch."""
+        """[(size, [(clip, data, ids)])]: whole clips, at most max_batch frames, one resolution per batch."""
         batches = []
         for size, clips in by_size.items():
             batch, used = [], 0
@@ -216,7 +202,7 @@ class NvdecClipAestheticStage(CuratorStage):
                 if used + len(ids) > self._max_batch:
                     batches.append((size, batch))
                     batch, used = [], 0
-                batch.append((clip, data, ids, used))
+                batch.append((clip, data, ids))
                 used += len(ids)
             if batch:
                 batches.append((size, batch))
@@ -226,27 +212,23 @@ class NvdecClipAestheticStage(CuratorStage):
         """Decode of batches k+1, k+2 (NVDEC + host parsing threads) overlaps preprocess + tower of batch k (SMs)."""
         seek, tower, stream = self._seek, self._model.tower, torch.cuda.current_stream()
         ring_pos: dict[tuple[int, int], int] = {}
-        slots_of, futs, inflight = {}, {}, {}
+        groups, inflight = {}, {}
         decoded = 0
-
-        def decode_one(dec, data, ids, pool, first):
-            return dec.decode(data, ids, pool, np.arange(first, first + len(ids), dtype=np.int32), seek_keyframes=seek)["frames_decoded"]
 
         def submit(k):
             size, items = batches[k]
             r = ring_pos.get(size, 0)
             ring_pos[size] = (r + 1) % self.RING
-            pool = self._pool(size, r)
-            slots_of[k] = (pool, k % self.RING)
-            futs[k] = [self._decode_pool.submit(decode_one, data, ids, pool, first, shape=size) for _, data, ids, first in items]
+            pool = self._pools.get(size, self._max_batch, r)
+            groups[k] = (pool, self._decode_pool.submit_group(pool, size, [(data, ids) for _, data, ids in items], seek))
 
         def finalize(k):
             """Batch k's results are on the host once its event has fired: write them onto the clips."""
-            ev, errs, n = inflight.pop(k)
+            ev, jobs, errs, n = inflight.pop(k)
             ev.synchronize()
             score_h, emb_h = self._host_buffers(k % self.RING)
             score_h = score_h[:n].numpy() if score_h is not None else None
-            for (clip, _, ids, first), err in zip(batches[k][1], errs):
+            for (clip, _, ids), (first, _), err in zip(batches[k][1], jobs, errs):
                 if err is not None:
                     self._decode_failed(clip, err)
                     continue
@@ -259,15 +241,10 @@ class NvdecClipAestheticStage(CuratorStage):
         for k in range(min(2, len(batches))):
             submit(k)
         for k in range(len(batches)):
-            errs = []
-            for f in futs.pop(k):
-                try:
-                    decoded += f.result()
-                    errs.append(None)
-                except CurateB200Error as e:
-                    errs.append(e)
-            pool, r = slots_of.pop(k)
-            n = sum(len(ids) for _, _, ids, _ in batches[k][1])
+            pool, jobs = groups.pop(k)
+            n_decoded, errs = collect_group(jobs)
+            decoded += n_decoded
+            n = sum(len(ids) for _, _, ids in batches[k][1])
             norm = {} if self._norm[0] is None else {"mean": self._norm[0], "std": self._norm[1]}
             if self._target_res is not None:
                 th, tw = self._target_res
@@ -275,14 +252,14 @@ class NvdecClipAestheticStage(CuratorStage):
                 emb, _, score = tower.embed_pool(self._ctx.rgb_pool(small), **norm)
             else:
                 emb, _, score = tower.embed_pool(pool, slots=np.arange(n, dtype=np.int32), **norm)
-            score_h, emb_h = self._host_buffers(r)
+            score_h, emb_h = self._host_buffers(k % self.RING)
             if score_h is not None:
                 score_h[:n].copy_(score, non_blocking=True)
             if emb_h is not None:
                 emb_h[:n].copy_(emb, non_blocking=True)
             ev = torch.cuda.Event()
             ev.record(stream)
-            inflight[k] = (ev, errs, n)
+            inflight[k] = (ev, jobs, errs, n)
             if k >= 1:
                 finalize(k - 1)  # also frees the surface pool and host buffers batch k+2 is about to reuse
             if k + 2 < len(batches):

@@ -19,7 +19,7 @@ from .._lib import CurateB200Error
 from ..data_model import StageTimer
 from ..interfaces import CuratorStage, CuratorStageResource, ModelInterface
 from ..models.internvideo2_frames import InternVideo2FrameFormulator, select_frame_ids
-from ..runtime import DecoderPool, alloc_nv12_pool, get_context, mp4_index
+from ..runtime import DecoderPool, SurfacePools, check_colour, collect_group, even_size, get_context, mp4_index
 from ..sampling import FrameExtractionPolicy, FrameExtractionSignature
 
 try:
@@ -66,10 +66,10 @@ class InternVideo2FrameCreationStage(CuratorStage):
         self._frame_extraction_signature = FrameExtractionSignature(extraction_policy=FrameExtractionPolicy.sequence, target_fps=target_fps).to_str()
         self._model = model if model is not None else InternVideo2FrameFormulator()
         self._verbose, self._log_stats = verbose, log_stats
-        self._source, self._colour, self._num_gpus = source, colour, num_gpus_per_worker
+        self._source, self._colour, self._num_gpus = source, check_colour(colour), num_gpus_per_worker
         self._num_decoders, self._stage_batch_size = num_decoders, stage_batch_size
         self._decode_pool = None
-        self._pools: dict[tuple, list] = {}
+        self._pools: SurfacePools | None = None
 
     @property
     def model(self) -> ModelInterface:
@@ -86,29 +86,20 @@ class InternVideo2FrameCreationStage(CuratorStage):
     def stage_setup(self) -> None:
         self._model.setup()
         self._ctx = get_context()
+        self._pools = SurfacePools(self._ctx, 2, self._model.get_target_num_frames(), self._colour)
 
     def destroy(self) -> None:
         if self._decode_pool is not None:
             self._decode_pool.close()
             self._decode_pool = None
-        self._pools.clear()
+        if self._pools is not None:
+            self._pools.clear()
 
     # ---- NVDEC side --------------------------------------------------------------------------------
     def _decoders(self) -> DecoderPool:
         if self._decode_pool is None:
             self._decode_pool = DecoderPool(self._ctx, self._num_decoders)
         return self._decode_pool
-
-    def _pool(self, size: tuple[int, int], r: int, n: int):
-        ring = self._pools.get(size)
-        if ring is None:
-            if len(self._pools) >= 4:
-                self._pools.pop(next(iter(self._pools)))
-            ring = self._pools[size] = [None, None]
-        if ring[r] is None or ring[r].buf.shape[0] < n:
-            ring[r] = None
-            ring[r] = alloc_nv12_pool(self._ctx, n, size[0], size[1], self._colour)
-        return ring[r]
 
     def _plan(self, clip, data):
         """-> (size, distinct frame ids to decode, slot of every kept frame relative to the clip's first slot), None when the
@@ -125,7 +116,7 @@ class InternVideo2FrameCreationStage(CuratorStage):
             logger.warning(f"Clip {clip.uuid} has <{fn} frames at target_fps={self._target_fps}; sampled at {fps}.")
         keep = np.asarray(ids)[select_frame_ids(len(ids), fn)]
         uniq, inverse = np.unique(keep, return_inverse=True)  # a frame kept twice (supersampled clip) is decoded once
-        return ((idx["width"] + 1) & ~1, (idx["height"] + 1) & ~1), uniq.astype(np.int32), inverse.astype(np.int32)
+        return even_size(idx["width"], idx["height"]), uniq.astype(np.int32), inverse.astype(np.int32)
 
     def _tubes_from_streams(self, items) -> None:
         """items: [(clip, data)].  Decode groups of GROUP clips on the session pool (group k+1 decodes while group k is
@@ -145,32 +136,21 @@ class InternVideo2FrameCreationStage(CuratorStage):
         groups = [(size, clips[i : i + self.GROUP]) for size, clips in by_size.items() for i in range(0, len(clips), self.GROUP)]
         ring_pos: dict[tuple, int] = {}
 
-        def decode_one(dec, data, ids, pool, first):
-            dec.decode(data, ids, pool, np.arange(first, first + len(ids), dtype=np.int32))
-
         def submit(k):
             size, clips = groups[k]
             r = ring_pos.get(size, 0)
             ring_pos[size] = r ^ 1
-            cap, need = fn, sum(len(ids) for _, _, ids, _ in clips)
-            while cap < need:
-                cap *= 2
-            pool = self._pool(size, r, cap)
-            futs, first = [], 0
-            for _, data, ids, _ in clips:
-                futs.append((first, self._decoders().submit(decode_one, data, ids, pool, first, shape=size)))
-                first += len(ids)
-            return pool, futs
+            pool = self._pools.get(size, sum(len(ids) for _, _, ids, _ in clips), r)
+            return pool, self._decoders().submit_group(pool, size, [(data, ids) for _, data, ids, _ in clips])
 
         pending = submit(0) if groups else None
         for k, (_, clips) in enumerate(groups):
-            pool, futs = pending
+            pool, jobs = pending
+            _, errs = collect_group(jobs)
             ok, slots = [], []
-            for (clip, _, _, inverse), (first, fut) in zip(clips, futs):
-                try:
-                    fut.result()
-                except CurateB200Error as e:
-                    self._decode_failed(clip, e)
+            for (clip, _, _, inverse), (first, _), err in zip(clips, jobs, errs):
+                if err is not None:
+                    self._decode_failed(clip, err)
                     continue
                 ok.append(clip)
                 slots.append(first + inverse)
