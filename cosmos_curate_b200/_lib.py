@@ -21,7 +21,7 @@ DT_F16, DT_BF16, DT_F32 = 0, 1, 2
 LAYOUT_NCHW, LAYOUT_PATCH = 0, 1
 ACT_QUICK_GELU, ACT_GELU_TANH = 0, 1
 ARCH_CLIP, ARCH_SIGLIP = 0, 1
-EPI_NONE, EPI_QUICK_GELU, EPI_GELU_TANH = 0, 1, 2
+EPI_NONE, EPI_QUICK_GELU, EPI_GELU_TANH, EPI_GELU_ERF = 0, 1, 2, 3
 DECODE_SEEK_SYNC, DECODE_DISCARD_ALL = 1, 2
 CUBIC_OPENCV, CUBIC_IPP = 0, 1
 
@@ -43,6 +43,13 @@ class VitCfg(C.Structure):
     _fields_ = [
         ("image_size", C.c_int), ("patch", C.c_int), ("hidden", C.c_int), ("layers", C.c_int), ("heads", C.c_int),
         ("mlp", C.c_int), ("proj_dim", C.c_int), ("act", C.c_int), ("arch", C.c_int), ("ln_eps", C.c_float),
+    ]  # fmt: skip
+
+
+class Iv2Cfg(C.Structure):
+    _fields_ = [
+        ("image_size", C.c_int), ("patch", C.c_int), ("frames", C.c_int), ("hidden", C.c_int), ("layers", C.c_int), ("heads", C.c_int),
+        ("mlp", C.c_int), ("clip_dim", C.c_int), ("embed_dim", C.c_int), ("rms_eps", C.c_float), ("ln_eps", C.c_float),
     ]  # fmt: skip
 
 
@@ -109,6 +116,15 @@ SIGNATURES = {
     "cb_gemm_f16": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _vp]),
     "cb_layernorm_f16": (_i, [_vp, _vp, _vp, _vp, _vp, _i, _i, _f, _vp]),
     "cb_attention_f16": (_i, [_vp, _vp, _vp, _i, _i, _i, _i, _vp]),
+    "cb_gemm_f16_ex": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _vp]),
+    "cb_rmsnorm_f16": (_i, [_vp, _vp, _vp, _vp, _i, _i, _f, _vp]),
+    "cb_qk_rmsnorm_f16": (_i, [_vp, _vp, _vp, _vp, _i, _i, _f, _vp]),
+    "cb_attention_stream_f16": (_i, [_vp, _vp, _vp, _i, _i, _i, _i, _vp]),
+    "cb_iv2_create": (_i, [_vp, C.POINTER(Iv2Cfg), C.POINTER(_vp)]),
+    "cb_iv2_destroy": (None, [_vp]),
+    "cb_iv2_set_tensor": (_i, [_vp, C.c_char_p, _pf, C.c_size_t]),
+    "cb_iv2_finalize": (_i, [_vp, _i]),
+    "cb_iv2_forward": (_i, [_vp, _vp, _i, _vp, _vp]),
 }
 
 _lib = None

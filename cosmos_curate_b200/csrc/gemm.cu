@@ -45,6 +45,7 @@ struct GemmArgs {
   const float* bias;  // [N] or null
   int M, N, K;
   int residual;  // nonzero: add the [M][N] fp32 tensor of map_r (fp32 output only)
+  const float* gamma;  // [N] per-column scale of (acc + bias), applied before the residual add (SCALE instantiations only)
 };
 
 // x * sigmoid(1.702 x) with one ex2.approx + one rcp.approx (both ~1 ulp; the result is rounded to fp16 anyway)
@@ -57,10 +58,14 @@ __device__ __forceinline__ float act_gelu_tanh(float x) {
   return 0.5f * x * (1.f + t);
 }
 
+// nn.GELU(): 0.5 x (1 + erf(x / sqrt(2))); CUDA's erff is within 2 ulp
+__device__ __forceinline__ float act_gelu_erf(float x) { return 0.5f * x * (1.f + erff(x * 0.7071067811865476f)); }
+
 template <int ACT>
 __device__ __forceinline__ float act(float x) {
   if (ACT == CB_EPI_QUICK_GELU) return act_quick_gelu(x);
   if (ACT == CB_EPI_GELU_TANH) return act_gelu_tanh(x);
+  if (ACT == CB_EPI_GELU_ERF) return act_gelu_erf(x);
   return x;
 }
 
@@ -71,8 +76,9 @@ __device__ __forceinline__ void wgmma_tile(float* d, uint64_t da, uint64_t db, i
 }
 
 // map_o: the output ([M][N] fp32 or fp16, box 128 bytes x 64 rows, 128-byte swizzle); map_r: the residual, same box (read only
-// when g.residual is set)
-template <int BN, int ACT, bool OUT_F32>
+// when g.residual is set).  SCALE (fp32 output only): out = residual + gamma * (acc + bias), LayerScale; gamma is read once per
+// tile beside the bias.
+template <int BN, int ACT, bool OUT_F32, bool SCALE = false>
 __global__ void __launch_bounds__(kGemmThreads, 1)
     gemm_wgmma_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b, const __grid_constant__ CUtensorMap map_o,
                       const __grid_constant__ CUtensorMap map_r, const GemmArgs g) {
@@ -145,6 +151,7 @@ __global__ void __launch_bounds__(kGemmThreads, 1)
     uint32_t phase = 0;
     float acc[BN / 2];
     float2 bias[BN / 8];
+    float2 gam[SCALE ? BN / 8 : 1];
     for (int t = first; t < num_tiles; t += step) {
       const int m_blk = t / n_tiles, n_blk = t % n_tiles;
       const int row0 = m_blk * BM + c * 64, col0 = n_blk * BN;
@@ -177,6 +184,7 @@ __global__ void __launch_bounds__(kGemmThreads, 1)
       for (int j = 0; j < BN / 8; ++j) {
         const int col = col0 + 8 * j + 2 * (lane & 3);
         bias[j] = (g.bias && col < g.N) ? __ldg((const float2*)(g.bias + col)) : make_float2(0.f, 0.f);
+        if (SCALE) gam[j] = col < g.N ? __ldg((const float2*)(g.gamma + col)) : make_float2(0.f, 0.f);
       }
       wgmma_wait<0>();
       release(prev);
@@ -202,6 +210,9 @@ __global__ void __launch_bounds__(kGemmThreads, 1)
           for (int h = 0; h < 2; ++h) {
             uint8_t* row = buf + (rl + 8 * h) * 128;
             float v0 = act<ACT>(acc[4 * j + 2 * h] + bias[j].x), v1 = act<ACT>(acc[4 * j + 2 * h + 1] + bias[j].y);
+            // LayerScale as its own rounded product (the reference's x + gamma * y in fp32): left contractible, the compiler fuses it
+            // into the residual add in some unrolled copies and not others, and a row's result would depend on its slot in the tile
+            if (SCALE) v0 = __fmul_rn(v0, gam[j].x), v1 = __fmul_rn(v1, gam[j].y);
             if (OUT_F32) {
               float2* p = (float2*)(row + (((2 * jj + ((lane & 3) >> 1)) ^ sw) << 4) + 8 * (lane & 1));
               if (has_res) {
@@ -232,11 +243,11 @@ __global__ void __launch_bounds__(kGemmThreads, 1)
   }
 }
 
-template <int BN, int ACT, bool OUT_F32>
+template <int BN, int ACT, bool OUT_F32, bool SCALE = false>
 static int launch_gemm(cb_ctx* ctx, const CUtensorMap& ma, const CUtensorMap& mb, const CUtensorMap& mo, const CUtensorMap& mr, const GemmArgs& g,
                        cudaStream_t stream) {
   using Cfg = GemmCfg<BN>;
-  auto kern = gemm_wgmma_kernel<BN, ACT, OUT_F32>;
+  auto kern = gemm_wgmma_kernel<BN, ACT, OUT_F32, SCALE>;
   static bool attr_done[64] = {};  // per template instantiation AND per device
   bool& attr_set = attr_done[ctx->device & 63];
   if (!attr_set) {
@@ -256,12 +267,14 @@ static int dispatch_gemm(cb_ctx* ctx, const CUtensorMap& ma, const CUtensorMap& 
   if (out_f32) return launch_gemm<BN, CB_EPI_NONE, true>(ctx, ma, mb, mo, mr, g, stream);
   if (epilogue == CB_EPI_QUICK_GELU) return launch_gemm<BN, CB_EPI_QUICK_GELU, false>(ctx, ma, mb, mo, mr, g, stream);
   if (epilogue == CB_EPI_GELU_TANH) return launch_gemm<BN, CB_EPI_GELU_TANH, false>(ctx, ma, mb, mo, mr, g, stream);
+  if (epilogue == CB_EPI_GELU_ERF) return launch_gemm<BN, CB_EPI_GELU_ERF, false>(ctx, ma, mb, mo, mr, g, stream);
   if (epilogue == CB_EPI_NONE) return launch_gemm<BN, CB_EPI_NONE, false>(ctx, ma, mb, mo, mr, g, stream);
   return fail(ctx, CB_ERR_ARG, "gemm: unknown epilogue %d", epilogue);
 }
 
-int gemm_f16(cb_ctx* ctx, const void* A, const void* W, const float* bias, const float* residual, float* out_f32, void* out_f16, int M,
-             int N, int K, int epilogue, cudaStream_t stream) {
+// gamma: nullable [N] LayerScale (fp32 output only); its tiles are 128 x 128 (the scale's registers sit beside the bias')
+int gemm_f16_ex(cb_ctx* ctx, const void* A, const void* W, const float* bias, const float* gamma, const float* residual, float* out_f32,
+                void* out_f16, int M, int N, int K, int epilogue, cudaStream_t stream) {
   if (!A || !W || (!out_f32 && !out_f16)) return fail(ctx, CB_ERR_ARG, "gemm: null operand");
   if (M <= 0 || N <= 0 || K <= 0) return fail(ctx, CB_ERR_ARG, "gemm: bad shape %dx%dx%d", M, N, K);
   if ((K & 7) || (N & 7)) return fail(ctx, CB_ERR_ARG, "gemm: N and K must be multiples of 8 (got N=%d K=%d)", N, K);
@@ -270,9 +283,11 @@ int gemm_f16(cb_ctx* ctx, const void* A, const void* W, const float* bias, const
   if (((uintptr_t)out | (uintptr_t)residual) & 15) return fail(ctx, CB_ERR_ARG, "gemm: output and residual must be 16-byte aligned");
   if (out_f32 && epilogue != CB_EPI_NONE) return fail(ctx, CB_ERR_UNSUPPORTED, "gemm: activation with fp32 output");
   if (residual && !out_f32) return fail(ctx, CB_ERR_UNSUPPORTED, "gemm: residual needs the fp32 output");
+  if (gamma && !out_f32) return fail(ctx, CB_ERR_UNSUPPORTED, "gemm: gamma needs the fp32 output");
+  if ((uintptr_t)gamma & 7) return fail(ctx, CB_ERR_ARG, "gemm: gamma must be 8-byte aligned");
   // 128 x 256 tiles when that still fills the machine, else 128 x 128
   const int tiles256 = ((M + BM - 1) / BM) * ((N + 255) / 256);
-  const bool wide = (N % 256 == 0 || N > 1024) && tiles256 >= ctx->sm_count;
+  const bool wide = !gamma && (N % 256 == 0 || N > 1024) && tiles256 >= ctx->sm_count;
   const int BN = wide ? 256 : 128;
   CUtensorMap ma, mb, mo, mr;
   uint64_t da[2] = {(uint64_t)K, (uint64_t)M}, db[2] = {(uint64_t)K, (uint64_t)N}, st[1] = {(uint64_t)K * 2};
@@ -290,12 +305,24 @@ int gemm_f16(cb_ctx* ctx, const void* A, const void* W, const float* bias, const
   if (rc) return rc;
   mr = mo;
   if (residual && (rc = make_tensor_map(ctx, &mr, dt, 2, residual, dout, sout, bout, CU_TENSOR_MAP_SWIZZLE_128B))) return rc;
-  GemmArgs g{bias, M, N, K, residual != nullptr};
+  GemmArgs g{bias, M, N, K, residual != nullptr, gamma};
+  if (gamma) return launch_gemm<128, CB_EPI_NONE, true, true>(ctx, ma, mb, mo, mr, g, stream);
   return BN == 256 ? dispatch_gemm<256>(ctx, ma, mb, mo, mr, g, out_f32 != nullptr, epilogue, stream)
                    : dispatch_gemm<128>(ctx, ma, mb, mo, mr, g, out_f32 != nullptr, epilogue, stream);
 }
 
+int gemm_f16(cb_ctx* ctx, const void* A, const void* W, const float* bias, const float* residual, float* out_f32, void* out_f16, int M,
+             int N, int K, int epilogue, cudaStream_t stream) {
+  return gemm_f16_ex(ctx, A, W, bias, nullptr, residual, out_f32, out_f16, M, N, K, epilogue, stream);
+}
+
 }  // namespace cb
+
+extern "C" int cb_gemm_f16_ex(cb_ctx* ctx, const void* A, const void* W, const float* bias, const float* gamma, const float* residual,
+                              float* out_f32, void* out_f16, int M, int N, int K, int epilogue, void* stream) {
+  if (!ctx) return CB_ERR_ARG;
+  return cb::gemm_f16_ex(ctx, A, W, bias, gamma, residual, out_f32, out_f16, M, N, K, epilogue, (cudaStream_t)stream);
+}
 
 extern "C" int cb_gemm_f16(cb_ctx* ctx, const void* A, const void* W, const float* bias, const float* residual, float* out_f32,
                            void* out_f16, int M, int N, int K, int epilogue, void* stream) {

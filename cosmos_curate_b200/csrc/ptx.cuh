@@ -80,6 +80,13 @@ __device__ __forceinline__ void tma_load_3d(void* dst, const CUtensorMap* m, uin
       "l"(m), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2)
       : "memory");
 }
+__device__ __forceinline__ void tma_load_5d(void* dst, const CUtensorMap* m, uint64_t* bar, int c0, int c1, int c2, int c3, int c4) {
+  asm volatile(
+      "cp.async.bulk.tensor.5d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6, %7}], [%2];" ::"r"(
+          smem_u32(dst)),
+      "l"(m), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "r"(c4)
+      : "memory");
+}
 // with an L2 cache-policy hint (createpolicy value)
 __device__ __forceinline__ void tma_load_2d_hint(void* dst, const CUtensorMap* m, uint64_t* bar, int c0, int c1, uint64_t policy) {
   asm volatile(

@@ -5,8 +5,12 @@
 //                          mma.sync m16n8k16 with fp32 online softmax (4 % of the tower's FLOPs; the dense
 //                          Linear layers are the wgmma kernel in gemm.cu)
 //   clip_tail_kernel       post_layernorm(CLS) -> visual_projection -> L2 normalise -> aesthetic affine head
+//   InternVideo2 tower:    rmsnorm_kernel (fp32 -> fp16), qk_rmsnorm_kernel (q and k thirds of the QKV rows, in place),
+//                          tube_patches_kernel (float32 tubes -> patch rows), token_mean_kernel, clip_pool_kernel (one query
+//                          per clip)
 #include <cuda_fp16.h>
 
+#include <algorithm>
 #include <type_traits>
 
 #include "common.h"
@@ -512,6 +516,168 @@ __global__ void __launch_bounds__(256) affine_score_kernel(const float* __restri
   if (lane == 0) out[row] = acc + b;
 }
 
+
+// ----------------------------------------------------------------------------------- InternVideo2 tower
+// RMSNorm (internvideo2.py:155-166): y = w * (x * rsqrt(mean(x^2) + eps)), statistics in fp32, one warp per row, d = 128 * chunks.
+template <int CHUNKS>
+__global__ void __launch_bounds__(256) rmsnorm_kernel(const float* __restrict__ x, const float* __restrict__ w, __half* __restrict__ y, int rows,
+                                                      int d, float eps) {
+  constexpr int kMax = CHUNKS > 0 ? CHUNKS : kLnMaxChunks;
+  const int row = blockIdx.x * 8 + (threadIdx.x >> 5), lane = threadIdx.x & 31;
+  if (row >= rows) return;
+  const int chunks = CHUNKS > 0 ? CHUNKS : d >> 7;
+  const float4* xr = (const float4*)(x + (size_t)row * d);
+  float4 v[kMax];
+  float s = 0.f;
+#pragma unroll
+  for (int i = 0; i < kMax; ++i)
+    if (i < chunks) {
+      v[i] = xr[lane + 32 * i];
+      s += (v[i].x * v[i].x + v[i].y * v[i].y) + (v[i].z * v[i].z + v[i].w * v[i].w);
+    }
+  const float r = rsqrtf(warp_sum(s) / (float)d + eps);
+#pragma unroll
+  for (int i = 0; i < kMax; ++i)
+    if (i < chunks) {
+      const float4 g = __ldg((const float4*)w + lane + 32 * i);
+      const __half2 h0 = __floats2half2_rn(v[i].x * r * g.x, v[i].y * r * g.y), h1 = __floats2half2_rn(v[i].z * r * g.z, v[i].w * r * g.w);
+      uint2 o;
+      o.x = *(const uint32_t*)&h0, o.y = *(const uint32_t*)&h1;
+      ((uint2*)(y + (size_t)row * d))[lane + 32 * i] = o;
+    }
+}
+
+// q_norm / k_norm of Attention (internvideo2.py:217-221): over all d columns of the row's q (part 0) or k (part 1) third, in place.
+// One warp per (row, part).
+template <int CHUNKS>
+__global__ void __launch_bounds__(256) qk_rmsnorm_kernel(__half* __restrict__ qkv, const float* __restrict__ wq, const float* __restrict__ wk,
+                                                         int rows, int d, float eps) {
+  constexpr int kMax = CHUNKS > 0 ? CHUNKS : kLnMaxChunks;
+  const int item = blockIdx.x * 8 + (threadIdx.x >> 5), lane = threadIdx.x & 31;
+  if (item >= 2 * rows) return;
+  const int row = item >> 1, part = item & 1;
+  const int chunks = CHUNKS > 0 ? CHUNKS : d >> 7;
+  uint2* p = (uint2*)(qkv + (size_t)row * 3 * d + (size_t)part * d);
+  const float* w = part ? wk : wq;
+  float4 v[kMax];
+  float s = 0.f;
+#pragma unroll
+  for (int i = 0; i < kMax; ++i)
+    if (i < chunks) {
+      const uint2 raw = p[lane + 32 * i];
+      const float2 a = __half22float2(*(const __half2*)&raw.x), b = __half22float2(*(const __half2*)&raw.y);
+      v[i] = make_float4(a.x, a.y, b.x, b.y);
+      s += (v[i].x * v[i].x + v[i].y * v[i].y) + (v[i].z * v[i].z + v[i].w * v[i].w);
+    }
+  const float r = rsqrtf(warp_sum(s) / (float)d + eps);
+#pragma unroll
+  for (int i = 0; i < kMax; ++i)
+    if (i < chunks) {
+      const float4 g = __ldg((const float4*)w + lane + 32 * i);
+      const __half2 h0 = __floats2half2_rn(v[i].x * r * g.x, v[i].y * r * g.y), h1 = __floats2half2_rn(v[i].z * r * g.z, v[i].w * r * g.w);
+      uint2 o;
+      o.x = *(const uint32_t*)&h0, o.y = *(const uint32_t*)&h1;
+      p[lane + 32 * i] = o;
+    }
+}
+
+// float32 tubes [frames][3][S][S] (frames = clips * T) -> fp16 patch rows [frames][(S/P)^2][k_pad], k = (c, y, x) zero-padded from
+// 3 P^2: the Conv3d(k = (1, P, P), stride = kernel) patch embed as a GEMM.  One thread per output pair.
+__global__ void __launch_bounds__(256) tube_patches_kernel(const float* __restrict__ tubes, __half* __restrict__ out, int frames, int S, int P,
+                                                           int k_pad) {
+  const int G = S / P, kp = 3 * P * P;
+  const size_t total = (size_t)frames * G * G * (k_pad / 2);
+  for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) {
+    const int k = (int)(i % (k_pad / 2)) * 2;
+    const size_t fp = i / (k_pad / 2);
+    const int patch = (int)(fp % (G * G));
+    const size_t f = fp / (G * G);
+    const int py = patch / G, px = patch - py * G;
+    float e[2];
+#pragma unroll
+    for (int q = 0; q < 2; ++q) {
+      const int kk = k + q;
+      if (kk < kp) {
+        const int c = kk / (P * P), r = kk - c * P * P, y = r / P, x = r - y * P;
+        e[q] = tubes[((f * 3 + c) * S + (py * P + y)) * (size_t)S + px * P + x];
+      } else {
+        e[q] = 0.f;
+      }
+    }
+    *(__half2*)(out + fp * k_pad + k) = __floats2half2_rn(e[0], e[1]);
+  }
+}
+
+// out[n][d] = mean over the T tokens of h[n][T][d] (AttentionPoolingBlock's x.mean(1)); fp32, tokens summed in order.
+__global__ void __launch_bounds__(128) token_mean_kernel(const float* __restrict__ h, float* __restrict__ out, int tokens, int d) {
+  const int col = blockIdx.x * blockDim.x + threadIdx.x, clip = blockIdx.y;
+  if (col >= d) return;
+  const float* x = h + (size_t)clip * tokens * d + col;
+  float s = 0.f;
+  for (int t = 0; t < tokens; ++t) s += x[(size_t)t * d];
+  out[(size_t)clip * d + col] = s / (float)tokens;
+}
+
+// Attention pooling with ONE query per clip (CrossAttention of AttentionPoolingBlock, internvideo2.py:72-101): per (clip, head)
+// softmax_t(scale q_h . k_t) applied to v_t.  q: fp32 [n][hidden] (unscaled), k, v: fp16 [n][tokens][hidden], out: fp16 [n][hidden].
+__global__ void __launch_bounds__(256) clip_pool_kernel(const float* __restrict__ q, const __half* __restrict__ k, const __half* __restrict__ v,
+                                                        __half* __restrict__ out, int tokens, int heads, int head_dim, float scale) {
+  extern __shared__ float sm_pool[];  // [tokens] probabilities, then [max(head_dim, slices * head_dim)] query / partial sums
+  float* prob = sm_pool;
+  float* qh = sm_pool + tokens;
+  __shared__ float red[32];
+  const int clip = blockIdx.x / heads, head = blockIdx.x - clip * heads;
+  const int hidden = heads * head_dim, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, nw = blockDim.x >> 5;
+  const size_t base = (size_t)clip * tokens * hidden + (size_t)head * head_dim;
+  for (int d = tid; d < head_dim; d += blockDim.x) qh[d] = q[(size_t)clip * hidden + head * head_dim + d] * scale;
+  __syncthreads();
+  float mx = -INFINITY;
+  for (int t = tid; t < tokens; t += blockDim.x) {
+    const __half* kr = k + base + (size_t)t * hidden;
+    float s = 0.f;
+    for (int d = 0; d < head_dim; d += 2) {
+      const float2 kk = __half22float2(*(const __half2*)(kr + d));
+      s = fmaf(kk.x, qh[d], fmaf(kk.y, qh[d + 1], s));
+    }
+    prob[t] = s;
+    mx = fmaxf(mx, s);
+  }
+  mx = warp_max(mx);
+  if (lane == 0) red[warp] = mx;
+  __syncthreads();
+  mx = red[0];
+  for (int i = 1; i < nw; ++i) mx = fmaxf(mx, red[i]);
+  __syncthreads();
+  float sum = 0.f;
+  for (int t = tid; t < tokens; t += blockDim.x) {
+    const float e = __expf(prob[t] - mx);
+    prob[t] = e;
+    sum += e;
+  }
+  sum = warp_sum(sum);
+  if (lane == 0) red[warp] = sum;
+  __syncthreads();
+  float tot = 0.f;
+  for (int i = 0; i < nw; ++i) tot += red[i];
+  const float inv = 1.f / tot;
+  const int slices = blockDim.x / head_dim > 0 ? blockDim.x / head_dim : 1;
+  float* part = qh;  // the query is dead: reuse for the per-slice partial sums
+  __syncthreads();
+  if (tid < slices * head_dim) {
+    const int d = tid % head_dim, sl = tid / head_dim;
+    const __half* vr = v + base + d;
+    float acc = 0.f;
+    for (int t = sl; t < tokens; t += slices) acc = fmaf(prob[t], __half2float(vr[(size_t)t * hidden]), acc);
+    part[sl * head_dim + d] = acc;
+  }
+  __syncthreads();
+  if (tid < head_dim) {
+    float acc = 0.f;
+    for (int sl = 0; sl < slices; ++sl) acc += part[sl * head_dim + tid];
+    out[(size_t)clip * hidden + head * head_dim + tid] = __float2half_rn(acc * inv);
+  }
+}
+
 // ------------------------------------------------------------------------------------------ host
 int affine_score(cb_ctx* ctx, const float* emb, const float* w, float b, float* out, int n, int d, cudaStream_t stream) {
   if (!emb || !w || !out) return fail(ctx, CB_ERR_ARG, "affine_score: null operand");
@@ -611,9 +777,78 @@ int clip_tail(cb_ctx* ctx, const float* h, size_t img_stride, const float* gamma
   return CB_OK;
 }
 
+
+int rmsnorm_f16(cb_ctx* ctx, const float* x, const float* w, void* y, int rows, int d, float eps, cudaStream_t stream) {
+  if (!x || !w || !y) return fail(ctx, CB_ERR_ARG, "rmsnorm: null operand");
+  if (rows < 0) return fail(ctx, CB_ERR_ARG, "rmsnorm: rows=%d", rows);
+  if (d <= 0 || d % 128 || d > 128 * kLnMaxChunks) return fail(ctx, CB_ERR_UNSUPPORTED, "rmsnorm: d=%d must be a multiple of 128 and <= %d", d, 128 * kLnMaxChunks);
+  if (rows == 0) return CB_OK;
+  mark_launch(ctx, CB_PROF_LAYERNORM, stream);
+  const unsigned grid = (unsigned)((rows + 7) / 8);
+  if (d >> 7 == 11)  // InternVideo2-1B, 1408
+    rmsnorm_kernel<11><<<grid, 256, 0, stream>>>(x, w, (__half*)y, rows, d, eps);
+  else
+    rmsnorm_kernel<0><<<grid, 256, 0, stream>>>(x, w, (__half*)y, rows, d, eps);
+  CB_CUDA(ctx, cudaGetLastError());
+  return CB_OK;
+}
+
+int qk_rmsnorm_f16(cb_ctx* ctx, void* qkv, const float* wq, const float* wk, int rows, int d, float eps, cudaStream_t stream) {
+  if (!qkv || !wq || !wk) return fail(ctx, CB_ERR_ARG, "qk_rmsnorm: null operand");
+  if (rows < 0) return fail(ctx, CB_ERR_ARG, "qk_rmsnorm: rows=%d", rows);
+  if (d <= 0 || d % 128 || d > 128 * kLnMaxChunks) return fail(ctx, CB_ERR_UNSUPPORTED, "qk_rmsnorm: d=%d must be a multiple of 128 and <= %d", d, 128 * kLnMaxChunks);
+  if (rows == 0) return CB_OK;
+  mark_launch(ctx, CB_PROF_LAYERNORM, stream);
+  const unsigned grid = (unsigned)((2 * (size_t)rows + 7) / 8);
+  if (d >> 7 == 11)
+    qk_rmsnorm_kernel<11><<<grid, 256, 0, stream>>>((__half*)qkv, wq, wk, rows, d, eps);
+  else
+    qk_rmsnorm_kernel<0><<<grid, 256, 0, stream>>>((__half*)qkv, wq, wk, rows, d, eps);
+  CB_CUDA(ctx, cudaGetLastError());
+  return CB_OK;
+}
+
+int tube_patches(cb_ctx* ctx, const float* tubes, void* out, int frames, int image_size, int patch, int k_pad, cudaStream_t stream) {
+  const int g = image_size / patch;
+  const size_t total = (size_t)frames * g * g * (k_pad / 2);
+  if (total == 0) return CB_OK;
+  mark_launch(ctx, CB_PROF_PREPROCESS, stream);
+  const unsigned grid = (unsigned)std::min<size_t>((total + 255) / 256, (size_t)ctx->sm_count * 16);
+  tube_patches_kernel<<<grid, 256, 0, stream>>>(tubes, (__half*)out, frames, image_size, patch, k_pad);
+  CB_CUDA(ctx, cudaGetLastError());
+  return CB_OK;
+}
+
+int token_mean(cb_ctx* ctx, const float* h, float* out, int n, int tokens, int d, cudaStream_t stream) {
+  mark_launch(ctx, CB_PROF_OTHER, stream);
+  token_mean_kernel<<<dim3((d + 127) / 128, n), 128, 0, stream>>>(h, out, tokens, d);
+  CB_CUDA(ctx, cudaGetLastError());
+  return CB_OK;
+}
+
+int clip_pool(cb_ctx* ctx, const float* q, const void* k, const void* v, void* out, int n, int tokens, int heads, int head_dim, cudaStream_t stream) {
+  const int threads = 256;
+  const int slices = threads / head_dim > 0 ? threads / head_dim : 1;
+  const size_t smem = (size_t)(tokens + std::max(1, slices) * head_dim) * sizeof(float);
+  if (smem > 48 * 1024) CB_CUDA(ctx, cudaFuncSetAttribute(clip_pool_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  mark_launch(ctx, CB_PROF_OTHER, stream);
+  clip_pool_kernel<<<n * heads, threads, smem, stream>>>(q, (const __half*)k, (const __half*)v, (__half*)out, tokens, heads, head_dim,
+                                                         1.0f / sqrtf((float)head_dim));
+  CB_CUDA(ctx, cudaGetLastError());
+  return CB_OK;
+}
+
 }  // namespace cb
 
 extern "C" {
+int cb_rmsnorm_f16(cb_ctx* ctx, const float* x, const float* weight, void* y, int rows, int d, float eps, void* stream) {
+  if (!ctx) return CB_ERR_ARG;
+  return cb::rmsnorm_f16(ctx, x, weight, y, rows, d, eps, (cudaStream_t)stream);
+}
+int cb_qk_rmsnorm_f16(cb_ctx* ctx, void* qkv, const float* q_weight, const float* k_weight, int rows, int d, float eps, void* stream) {
+  if (!ctx) return CB_ERR_ARG;
+  return cb::qk_rmsnorm_f16(ctx, qkv, q_weight, k_weight, rows, d, eps, (cudaStream_t)stream);
+}
 int cb_affine_score(cb_ctx* ctx, const float* emb, const float* w, float b, float* out, int n, int d, void* stream) {
   if (!ctx) return CB_ERR_ARG;
   return cb::affine_score(ctx, emb, w, b, out, n, d, (cudaStream_t)stream);

@@ -13,7 +13,7 @@ import numpy as np
 import torch
 
 from . import _lib
-from ._lib import SurfacePool, VitCfg, check
+from ._lib import Iv2Cfg, SurfacePool, VitCfg, check
 
 try:
     from loguru import logger
@@ -216,6 +216,44 @@ class Context(_Handle):
               "cb_gemm_f16", self.h)  # fmt: skip
         return out
 
+    def gemm_ex(self, a: torch.Tensor, w: torch.Tensor, bias=None, gamma=None, residual=None, epilogue: int = _lib.EPI_NONE,
+                out_f32: bool = False) -> torch.Tensor:
+        """cb_gemm_f16_ex: gemm() plus the per-column LayerScale `gamma` (fp32 output)."""
+        m, k = a.shape
+        n = w.shape[0]
+        assert a.dtype == torch.float16 and w.dtype == torch.float16 and w.shape[1] == k and a.is_contiguous() and w.is_contiguous()
+        if out_f32:
+            out = residual if residual is not None else torch.empty((m, n), dtype=torch.float32, device=a.device)
+            o32, o16 = out.data_ptr(), None
+        else:
+            out = torch.empty((m, n), dtype=torch.float16, device=a.device)
+            o32, o16 = None, out.data_ptr()
+        ptr = lambda t: t.data_ptr() if t is not None else None  # noqa: E731
+        check(self.lib.cb_gemm_f16_ex(self.h, a.data_ptr(), w.data_ptr(), ptr(bias), ptr(gamma), ptr(residual), o32, o16, m, n, k, epilogue,
+                                      _stream_ptr()), "cb_gemm_f16_ex", self.h)  # fmt: skip
+        return out
+
+    def rmsnorm(self, x: torch.Tensor, weight: torch.Tensor, eps: float) -> torch.Tensor:
+        rows, d = x.shape
+        y = torch.empty((rows, d), dtype=torch.float16, device=x.device)
+        check(self.lib.cb_rmsnorm_f16(self.h, x.data_ptr(), weight.data_ptr(), y.data_ptr(), rows, d, eps, _stream_ptr()), "cb_rmsnorm_f16", self.h)
+        return y
+
+    def qk_rmsnorm_(self, qkv: torch.Tensor, q_weight: torch.Tensor, k_weight: torch.Tensor, eps: float) -> torch.Tensor:
+        """In place on fp16 qkv [rows][3 * d]."""
+        rows, three_d = qkv.shape
+        check(self.lib.cb_qk_rmsnorm_f16(self.h, qkv.data_ptr(), q_weight.data_ptr(), k_weight.data_ptr(), rows, three_d // 3, eps, _stream_ptr()),
+              "cb_qk_rmsnorm_f16", self.h)  # fmt: skip
+        return qkv
+
+    def attention_stream(self, qkv: torch.Tensor, heads: int) -> torch.Tensor:
+        n, t, three_d = qkv.shape
+        d = three_d // 3
+        out = torch.empty((n, t, d), dtype=torch.float16, device=qkv.device)
+        check(self.lib.cb_attention_stream_f16(self.h, qkv.data_ptr(), out.data_ptr(), n, t, heads, d // heads, _stream_ptr()),
+              "cb_attention_stream_f16", self.h)  # fmt: skip
+        return out
+
     def layernorm(self, x: torch.Tensor, gamma: torch.Tensor, beta: torch.Tensor, eps: float) -> torch.Tensor:
         rows, d = x.shape
         y = torch.empty((rows, d), dtype=torch.float16, device=x.device)
@@ -305,6 +343,37 @@ class VitTower(_Handle):
                                              feat.data_ptr() if feat is not None else None, score.data_ptr() if score is not None else None,
                                              _stream_ptr()), "cb_vit_embed_surfaces", self.ctx.h)  # fmt: skip
         return emb, feat, score
+
+
+class Iv2Tower(_Handle):
+    """cb_iv2_* wrapper: weights in (fp32 numpy, names of include/curate_b200.h cb_iv2_set_tensor), clip embeddings out."""
+
+    FIELDS = ("image_size", "patch", "frames", "hidden", "layers", "heads", "mlp", "clip_dim", "embed_dim", "rms_eps", "ln_eps")
+
+    def __init__(self, ctx: Context, cfg: dict, weights: dict, max_clips: int = 8):
+        self.ctx, self.lib = ctx, ctx.lib
+        self.cfg = {k: cfg[k] for k in self.FIELDS}
+        h = C.c_void_p()
+        check(self.lib.cb_iv2_create(ctx.h, C.byref(Iv2Cfg(*[self.cfg[k] for k in self.FIELDS])), C.byref(h)), "cb_iv2_create", ctx.h)
+        self.h = h
+        ctx._children.add(self)
+        for name, arr in weights.items():
+            a = np.ascontiguousarray(arr, dtype=np.float32)
+            check(self.lib.cb_iv2_set_tensor(self.h, name.encode(), a.ctypes.data_as(C.POINTER(C.c_float)), a.size), f"cb_iv2_set_tensor({name})", ctx.h)
+        check(self.lib.cb_iv2_finalize(self.h, max_clips), "cb_iv2_finalize", ctx.h)
+        self.frames, self.embed_dim, self.max_clips = self.cfg["frames"], self.cfg["embed_dim"], max_clips
+
+    def _destroy(self):
+        self.lib.cb_iv2_destroy(self.h)
+
+    def forward(self, tubes: torch.Tensor) -> torch.Tensor:
+        """float32 cuda [n, frames, 3, S, S] -> unit-norm float32 cuda [n, embed_dim]."""
+        s = self.cfg["image_size"]
+        assert tubes.is_cuda and tubes.dtype == torch.float32 and tuple(tubes.shape[1:]) == (self.frames, 3, s, s), (tubes.dtype, tubes.shape)
+        tubes = tubes.contiguous()
+        out = torch.empty((tubes.shape[0], self.embed_dim), dtype=torch.float32, device=tubes.device)
+        check(self.lib.cb_iv2_forward(self.h, tubes.data_ptr(), tubes.shape[0], out.data_ptr(), _stream_ptr()), "cb_iv2_forward", self.ctx.h)
+        return out
 
 
 class ShotNet(_Handle):

@@ -10,6 +10,7 @@ Same-name drop-ins (constructor arguments, task mutations and error convention o
     FixedStrideExtractorStage   cosmos_curate/pipelines/video/clipping/clip_extraction_stages.py:664-760 (host only)
     ClipWriterStage             cosmos_curate/pipelines/video/read_write/metadata_writer_stage.py:66-1020 (local output directory, host only)
     InternVideo2FrameCreationStage  cosmos_curate/pipelines/video/embedding/internvideo2_stages.py:43-184 (the tower's input tube)
+    InternVideo2EmbeddingStage  cosmos_curate/pipelines/video/embedding/internvideo2_stages.py:187-309 (the 1B vision tower; no text tower)
     ClipFrameEmbeddingStage     local producer of clip.openai_embedding (the slot of embedding/openai_embedding_stage.py:47-190)
 New fused stage (replaces ClipFrameExtractionStage -> AestheticFilterStage [-> clip embedding] in one GPU pass):
     NvdecClipAestheticStage
@@ -25,6 +26,7 @@ from .download import VideoDownloader  # noqa: F401
 from .fixed_stride import FixedStrideExtractorStage  # noqa: F401
 from .fused_clip import NvdecClipAestheticStage  # noqa: F401
 from .frame_extraction import ClipFrameExtractionStage, VideoFrameExtractionStage  # noqa: F401
+from .internvideo2_embedding import InternVideo2EmbeddingStage  # noqa: F401
 from .internvideo2_frames import InternVideo2FrameCreationStage  # noqa: F401
 from .image_embedding import ImageCLIPEmbeddingStage  # noqa: F401
 from .transnetv2_extraction import NvdecShotDetectionStage, TransNetV2ClipExtractionStage  # noqa: F401

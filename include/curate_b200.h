@@ -280,6 +280,7 @@ int cb_cluster_sums(cb_ctx* ctx, const float* x, const long long* order, const l
 #define CB_EPI_NONE 0       /* C = A W^T (+ bias) */
 #define CB_EPI_QUICK_GELU 1 /* C = quick_gelu(A W^T + bias) */
 #define CB_EPI_GELU_TANH 2  /* C = gelu_tanh(A W^T + bias) */
+#define CB_EPI_GELU_ERF 3   /* C = gelu(A W^T + bias), the exact erf form (nn.GELU()) */
 /* C[M][N] = epilogue(A[M][K] . W[N][K]^T + bias[N]) (+ residual).  A, W fp16 row-major (K contiguous,
  * K % 8 == 0); bias fp32 or NULL.  If out_f32 != NULL: out_f32[M][N] (fp32) = result + (residual ?
  * residual[M][N] : 0) - residual may alias out_f32.  Else out_f16[M][N] = fp16(result).
@@ -292,6 +293,43 @@ int cb_layernorm_f16(cb_ctx* ctx, const float* x, const float* gamma, const floa
 /* Multi-head self-attention over qkv fp16 [n][tokens][3*hidden] (q | k | v, heads contiguous):
  * out fp16 [n][tokens][hidden]; softmax in fp32, scale = head_dim^-1/2. */
 int cb_attention_f16(cb_ctx* ctx, const void* qkv, void* out, int n, int tokens, int heads, int head_dim, void* stream);
+/* cb_gemm_f16 plus an optional per-column fp32 scale (LayerScale, internvideo2.py:169-183): with gamma != NULL (fp32 output only),
+ * out_f32 = (residual ? residual : 0) + gamma[N] * (A W^T + bias).  gamma is not folded into the fp16 weights. */
+int cb_gemm_f16_ex(cb_ctx* ctx, const void* A, const void* W, const float* bias, const float* gamma, const float* residual, float* out_f32,
+                   void* out_f16, int M, int N, int K, int epilogue, void* stream);
+/* y[rows][d] fp16 = weight * (x * rsqrt(mean(x^2) + eps)), statistics in fp32: RMSNorm of internvideo2.py:155-166.  d % 128 == 0. */
+int cb_rmsnorm_f16(cb_ctx* ctx, const float* x, const float* weight, void* y, int rows, int d, float eps, void* stream);
+/* In place on qkv fp16 [rows][3*d]: the q third of each row becomes RMSNorm(q) * q_weight and the k third RMSNorm(k) * k_weight, each
+ * over all d columns (every head together), fp32 statistics (Attention.qk_normalization, internvideo2.py:217-221).  d % 128 == 0. */
+int cb_qk_rmsnorm_f16(cb_ctx* ctx, void* qkv, const float* q_weight, const float* k_weight, int rows, int d, float eps, void* stream);
+/* Streamed attention for head_dim 88 (InternVideo2-1B: 16 heads of 88, T = 1025 at 4 frames): same layout and result as
+ * cb_attention_f16 (qkv fp16 [n][tokens][3*hidden] -> out fp16 [n][tokens][hidden], scale head_dim^-1/2).  Any other head_dim:
+ * CB_ERR_UNSUPPORTED.  n == 0 is a no-op. */
+int cb_attention_stream_f16(cb_ctx* ctx, const void* qkv, void* out, int n, int tokens, int heads, int head_dim, void* stream);
+
+/* ---- InternVideo2 video tower (clip embeddings) ------------------------------------------------------ */
+/* The vision half of InternVideo2_Stage2.get_vid_feat (models/internvideo2_mm.py:203-217): PretrainInternVideo2.forward
+ * (internvideo2.py:596-651) up to the attention-pooling clip_projector, then vision_proj and the L2 norm. */
+typedef struct cb_iv2 cb_iv2;
+typedef struct cb_iv2_cfg {
+  int image_size, patch, frames; /* 224, 14, 4: tokens = frames * (image_size / patch)^2 + 1 */
+  int hidden, layers, heads, mlp; /* 1408, 40, 16, 6144 (head_dim 88 only) */
+  int clip_dim, embed_dim;        /* clip_projector output 768, vision_proj output 512 */
+  float rms_eps, ln_eps;          /* 1e-6 (block and q/k RMSNorms), 1e-5 (pooling LayerNorms) */
+} cb_iv2_cfg;
+int cb_iv2_create(cb_ctx* ctx, const cb_iv2_cfg* cfg, cb_iv2** out);
+void cb_iv2_destroy(cb_iv2* iv2);
+/* Upload one named tensor (host fp32, row-major, `count` elements).  Names: patch_w[hidden][3*p*p] (Conv3d weight, k = (c, y, x)),
+ * patch_b, cls, pos[tokens][hidden], L<i>.{norm1_w, qkv_w[3h][h], q_norm_w, k_norm_w, proj_w[h][h], proj_b, ls1, norm2_w,
+ * fc1_w[mlp][h], fc1_b, fc2_w[h][mlp], fc2_b, ls2}, pool.{norm_q_w, norm_q_b, norm_k_w, norm_k_b, norm_v_w, norm_v_b, q_w[h][h], q_b,
+ * k_w, k_b, v_w, v_b, proj_w[clip_dim][h], proj_b}, vproj_w[embed_dim][clip_dim], vproj_b.  GEMM weights are stored as fp16; norms,
+ * biases, LayerScale gammas, cls and pos stay fp32. */
+int cb_iv2_set_tensor(cb_iv2* iv2, const char* name, const float* data, size_t count);
+/* Checks that every tensor arrived and sizes the workspace for batches of up to max_clips clips. */
+int cb_iv2_finalize(cb_iv2* iv2, int max_clips);
+/* tubes: device fp32 [n][frames][3][image_size][image_size] (InternVideo2FrameCreationStage's tubes); emb_out: device fp32
+ * [n][embed_dim], unit norm.  Clips are independent: an embedding does not depend on the other clips of the call. */
+int cb_iv2_forward(cb_iv2* iv2, const float* tubes, int n, float* emb_out, void* stream);
 
 #ifdef __cplusplus
 }
