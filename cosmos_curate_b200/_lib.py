@@ -14,7 +14,7 @@ PKG = Path(__file__).resolve().parent
 LIB_PATH = PKG / "libcurate_b200.so"
 
 CB_OK = 0
-CB_ERR = {-1: "CB_ERR_CUDA", -2: "CB_ERR_ARG", -3: "CB_ERR_UNSUPPORTED", -4: "CB_ERR_NVDEC", -5: "CB_ERR_DEMUX", -6: "CB_ERR_STATE"}
+CB_ERR = {-1: "CB_ERR_CUDA", -2: "CB_ERR_ARG", -3: "CB_ERR_UNSUPPORTED", -4: "CB_ERR_NVDEC", -5: "CB_ERR_DEMUX", -6: "CB_ERR_STATE", -7: "CB_ERR_INVALID"}
 ROWDOT_UPPER, ROWDOT_CLIP = 1, 2
 FMT_NV12, FMT_RGB24, FMT_NV12_SWS = 0, 1, 2
 DT_F16, DT_BF16, DT_F32 = 0, 1, 2
@@ -50,6 +50,13 @@ class Iv2Cfg(C.Structure):
     _fields_ = [
         ("image_size", C.c_int), ("patch", C.c_int), ("frames", C.c_int), ("hidden", C.c_int), ("layers", C.c_int), ("heads", C.c_int),
         ("mlp", C.c_int), ("clip_dim", C.c_int), ("embed_dim", C.c_int), ("rms_eps", C.c_float), ("ln_eps", C.c_float),
+    ]  # fmt: skip
+
+
+class Iv2TextCfg(C.Structure):
+    _fields_ = [
+        ("hidden", C.c_int), ("layers", C.c_int), ("heads", C.c_int), ("mlp", C.c_int), ("vocab", C.c_int), ("max_pos", C.c_int),
+        ("embed_dim", C.c_int), ("ln_eps", C.c_float),
     ]  # fmt: skip
 
 
@@ -125,6 +132,14 @@ SIGNATURES = {
     "cb_iv2_set_tensor": (_i, [_vp, C.c_char_p, _pf, C.c_size_t]),
     "cb_iv2_finalize": (_i, [_vp, _i]),
     "cb_iv2_forward": (_i, [_vp, _vp, _i, _vp, _vp]),
+    "cb_attention_masked_f16": (_i, [_vp, _vp, _vp, _i, _i, _i, _i, _vp, _vp]),
+    "cb_layernorm_post_f16": (_i, [_vp, _vp, _vp, _vp, _vp, _i, _i, _f, _vp]),
+    "cb_text_embed": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _vp]),
+    "cb_iv2_text_create": (_i, [_vp, C.POINTER(Iv2TextCfg), C.POINTER(_vp)]),
+    "cb_iv2_text_destroy": (None, [_vp]),
+    "cb_iv2_text_set_tensor": (_i, [_vp, C.c_char_p, _pf, C.c_size_t]),
+    "cb_iv2_text_finalize": (_i, [_vp, _i, _i]),
+    "cb_iv2_text_forward": (_i, [_vp, _pi32, _pi32, _i, _i, _vp, _vp]),
 }
 
 _lib = None

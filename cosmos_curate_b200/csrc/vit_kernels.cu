@@ -8,6 +8,8 @@
 //   InternVideo2 tower:    rmsnorm_kernel (fp32 -> fp16), qk_rmsnorm_kernel (q and k thirds of the QKV rows, in place),
 //                          tube_patches_kernel (float32 tubes -> patch rows), token_mean_kernel, clip_pool_kernel (one query
 //                          per clip)
+//   BERT text tower:       layernorm_post_kernel (post-LN: fp32 rows normalised in place + fp16 copy), attention_kernel<64, false, true>
+//                          (per-sequence key lengths)
 #include <cuda_fp16.h>
 
 #include <algorithm>
@@ -36,9 +38,12 @@ constexpr int kLnMaxChunks = 12;  // D <= 1536
 // CHUNKS > 0: the row length is the compile-time constant 128 * CHUNKS (the towers' widths get their own instantiation: the
 // register array is exactly the row, 46 instead of 78 registers at 1024, so more rows are in flight per SM); CHUNKS == 0: any
 // multiple of 128 up to 128 * kLnMaxChunks.  Same operations in the same order either way.
-template <bool OUT_F16, int CHUNKS = 0>
+// ALSO_F32 (with OUT_F16): the fp32 result goes to y32 as well; y32 may be x (every element of the row is loaded before the row
+// statistics, and every store depends on them).
+template <bool OUT_F16, int CHUNKS = 0, bool ALSO_F32 = false>
 __device__ __forceinline__ void ln_row(const float* __restrict__ x, const float* __restrict__ gamma, const float* __restrict__ beta,
-                                       void* __restrict__ y, int d, float eps, int lane, const float* __restrict__ add = nullptr) {
+                                       void* __restrict__ y, int d, float eps, int lane, const float* __restrict__ add = nullptr,
+                                       float* y32 = nullptr) {
   constexpr int kMax = CHUNKS > 0 ? CHUNKS : kLnMaxChunks;
   float4 v[kMax];
   const int chunks = CHUNKS > 0 ? CHUNKS : d >> 7;  // 128 floats per warp pass
@@ -73,6 +78,7 @@ __device__ __forceinline__ void ln_row(const float* __restrict__ x, const float*
         uint2 o;
         o.x = *(const uint32_t*)&h0, o.y = *(const uint32_t*)&h1;
         ((uint2*)y)[lane + 32 * i] = o;
+        if (ALSO_F32) ((float4*)y32)[lane + 32 * i] = make_float4(o0, o1, o2, o3);
       } else {
         ((float4*)y)[lane + 32 * i] = make_float4(o0, o1, o2, o3);
       }
@@ -85,6 +91,16 @@ __global__ void __launch_bounds__(256, MINB) layernorm_kernel(const float* __res
   const int row = blockIdx.x * 8 + (threadIdx.x >> 5);
   if (row >= rows) return;
   ln_row<true, CHUNKS>(x + (size_t)row * d, gamma, beta, y + (size_t)row * d, d, eps, threadIdx.x & 31);
+}
+
+// Post-LN (BERT's LayerNorm(x + sublayer(x)), the sum already in h): h = LayerNorm(h) in place, y = fp16 copy for the next GEMM.
+template <int CHUNKS, int MINB>
+__global__ void __launch_bounds__(256, MINB) layernorm_post_kernel(float* h, const float* __restrict__ gamma, const float* __restrict__ beta,
+                                                                   __half* __restrict__ y, int rows, int d, float eps) {
+  const int row = blockIdx.x * 8 + (threadIdx.x >> 5);
+  if (row >= rows) return;
+  float* x = h + (size_t)row * d;
+  ln_row<true, CHUNKS, true>(x, gamma, beta, y + (size_t)row * d, d, eps, threadIdx.x & 31, nullptr, x);
 }
 
 // ------------------------------------------------------------------------------- token assembly
@@ -155,11 +171,16 @@ __device__ __forceinline__ void prefetch_l2(const void* p) { asm volatile("prefe
 //   STREAM = false: one CTA per (image, head), all keys resident, warps loop over the query tiles      (T = 50, 257, ...)
 //   STREAM = true : grid.y splits the query tiles (one per warp), keys stream through shared memory in
 //                   blocks of kStreamKeys, the softmax state stays in registers across blocks             (T = 729, ...)
+//   MASKED = true : (resident only) image i is a sequence of lengths[i] <= tokens tokens padded to `tokens`: it runs exactly as an
+//                   unpadded sequence of lengths[i] tokens would (same tiles, chunks and masks; keys past the length are never loaded,
+//                   their shared-memory rows are zeros, so no padded V row enters P.V), and its output rows past the length are zeros.
 constexpr int kStreamKeys = 256;
 
-template <int HD, bool STREAM>
+template <int HD, bool STREAM, bool MASKED = false>
 __global__ void __launch_bounds__(kAttnThreads, 2) attention_kernel(const __half* __restrict__ qkv, __half* __restrict__ out, int tokens,
-                                                                     int heads, int head_dim, float scale_log2e) {
+                                                                     int heads, int head_dim, float scale_log2e,
+                                                                     const int* __restrict__ lengths = nullptr) {
+  static_assert(!(MASKED && STREAM), "the masked variant keeps every key resident");
   constexpr int PITCH = HD + 8;  // halves; 16-byte row skew keeps ldmatrix conflict-free
   constexpr int KS = HD / 16;    // k-steps over the head dimension
   extern __shared__ __align__(16) uint8_t smem_attn[];
@@ -172,17 +193,20 @@ __global__ void __launch_bounds__(kAttnThreads, 2) attention_kernel(const __half
   const size_t row_stride = (size_t)3 * hidden;
   const __half* base = qkv + (size_t)img * tokens * row_stride + (size_t)head * head_dim;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, g = lane >> 2, t4 = lane & 3;
+  // the sequence this CTA computes: `len` tokens, padded to `len_pad` (the whole image unless MASKED)
+  const int len = MASKED ? min(max(lengths[img], 0), tokens) : tokens;  // a length outside [0, tokens] cannot reach another image
+  const int len_pad = MASKED ? (len + 15) & ~15 : t_pad;
 
   // keys [k0, k0 + blk) (zero padded in both directions) -> shared memory, all copies in flight at once
   constexpr int VEC = HD / 8;
   const int vec_valid = head_dim / 8;  // head_dim % 8 == 0 is checked on the host
   auto load_block = [&](int k0) {
-    const int rows = min(blk, t_pad - k0);
+    const int rows = min(blk, len_pad - k0);
     for (int i = threadIdx.x; i < rows * VEC; i += kAttnThreads) {
       const int r = i / VEC, c = i - r * VEC;
       __half* dk = sK + (size_t)r * PITCH + c * 8;
       __half* dv = sV + (size_t)r * PITCH + c * 8;
-      if (k0 + r < tokens && c < vec_valid) {
+      if (k0 + r < len && c < vec_valid) {
         const __half* p = base + (size_t)(k0 + r) * row_stride + c * 8;
         cp_async_16(dk, p + hidden);
         cp_async_16(dv, p + 2 * hidden);
@@ -201,7 +225,7 @@ __global__ void __launch_bounds__(kAttnThreads, 2) attention_kernel(const __half
   using Full = std::integral_constant<int, 4>;
   using Tail = std::integral_constant<int, 2>;
 
-  const int q_tiles = t_pad >> 4;
+  const int q_tiles = len_pad >> 4;
   const int qt_first = STREAM ? (int)blockIdx.y * kAttnWarps + warp : warp;
   const int qt_step = STREAM ? q_tiles : kAttnWarps;  // STREAM: exactly one tile per warp (maybe none)
   bool first = true;
@@ -210,7 +234,7 @@ __global__ void __launch_bounds__(kAttnThreads, 2) attention_kernel(const __half
     // Q fragments straight from global memory (rows clamped; padded columns read as zero)
     uint32_t qa[KS][4];
     const int qrow = active ? qt * 16 : 0;
-    const int r0 = min(qrow + g, tokens - 1), r1 = min(qrow + g + 8, tokens - 1);
+    const int r0 = min(qrow + g, len - 1), r1 = min(qrow + g + 8, len - 1);
 #pragma unroll
     for (int ks = 0; ks < KS; ++ks) {
       const int c0 = ks * 16 + t4 * 2, c1 = c0 + 8;
@@ -220,7 +244,7 @@ __global__ void __launch_bounds__(kAttnThreads, 2) attention_kernel(const __half
       qa[ks][3] = c1 < head_dim ? __ldg((const uint32_t*)(base + (size_t)r1 * row_stride + c1)) : 0u;
     }
     if (!STREAM && qt + kAttnWarps < q_tiles) {  // pull the next tile's Q rows towards L2 while this tile computes
-      const int rn = min((qt + kAttnWarps) * 16 + (lane & 15), tokens - 1);
+      const int rn = min((qt + kAttnWarps) * 16 + (lane & 15), len - 1);
       prefetch_l2(base + (size_t)rn * row_stride);
     }
     if (!STREAM && first) {  // the Q loads above overlap the K/V fill
@@ -263,12 +287,12 @@ __global__ void __launch_bounds__(kAttnThreads, 2) attention_kernel(const __half
       constexpr int NKT = decltype(nkt_c)::value;
       float sc[4][4];
       qk_chunk(srow, nkt_c, sc);
-      if (kc + NKT * 8 > tokens) {  // padded keys only live in the last chunk(s)
+      if (kc + NKT * 8 > len) {  // padded keys only live in the last chunk(s)
 #pragma unroll
         for (int i = 0; i < NKT; ++i) {
           const int key = kc + i * 8 + t4 * 2;
-          if (key >= tokens) sc[i][0] = sc[i][2] = -INFINITY;
-          if (key + 1 >= tokens) sc[i][1] = sc[i][3] = -INFINITY;
+          if (key >= len) sc[i][0] = sc[i][2] = -INFINITY;
+          if (key + 1 >= len) sc[i][1] = sc[i][3] = -INFINITY;
         }
       }
       float mx0 = m0, mx1 = m1;
@@ -313,7 +337,7 @@ __global__ void __launch_bounds__(kAttnThreads, 2) attention_kernel(const __half
       }
     };
 
-    for (int k0 = 0; k0 < t_pad; k0 += blk) {  // one iteration when the keys are resident
+    for (int k0 = 0; k0 < len_pad; k0 += blk) {  // one iteration when the keys are resident
       if (STREAM) {
         __syncthreads();  // every warp is done with the previous block
         load_block(k0);
@@ -321,7 +345,7 @@ __global__ void __launch_bounds__(kAttnThreads, 2) attention_kernel(const __half
         __syncthreads();
       }
       if (active) {
-        const int rows = min(blk, t_pad - k0), full_end = rows & ~31;
+        const int rows = min(blk, len_pad - k0), full_end = rows & ~31;
         for (int r = 0; r < full_end; r += 32) pv_chunk(k0 + r, r, Full{});
         if (full_end < rows) pv_chunk(k0 + full_end, full_end, Tail{});
       }
@@ -340,14 +364,21 @@ __global__ void __launch_bounds__(kAttnThreads, 2) attention_kernel(const __half
     for (int d = 0; d < HD / 8; ++d) {
       const int c = d * 8 + t4 * 2;
       if (c < head_dim) {
-        if (row0 < tokens) *(uint32_t*)(ob + (size_t)row0 * hidden + c) = pack_half2(o[d][0] * inv0, o[d][1] * inv0);
-        if (row1 < tokens) *(uint32_t*)(ob + (size_t)row1 * hidden + c) = pack_half2(o[d][2] * inv1, o[d][3] * inv1);
+        if (row0 < len) *(uint32_t*)(ob + (size_t)row0 * hidden + c) = pack_half2(o[d][0] * inv0, o[d][1] * inv0);
+        if (row1 < len) *(uint32_t*)(ob + (size_t)row1 * hidden + c) = pack_half2(o[d][2] * inv1, o[d][3] * inv1);
       }
     }
   }
   if (!STREAM && first) {  // a warp without a tile (q_tiles < warps) still has to meet the fill barrier
     cp_async_wait_all();
     __syncthreads();
+  }
+  if (MASKED) {  // query rows past the length: zeros (finite, never read)
+    __half* ob = out + (size_t)img * tokens * hidden + (size_t)head * head_dim;
+    for (int i = threadIdx.x; i < (tokens - len) * (head_dim / 2); i += kAttnThreads) {
+      const int r = len + i / (head_dim / 2), c = 2 * (i % (head_dim / 2));
+      *(uint32_t*)(ob + (size_t)r * hidden + c) = 0u;
+    }
   }
 }
 
@@ -704,6 +735,21 @@ int layernorm_f16(cb_ctx* ctx, const float* x, const float* gamma, const float* 
   return CB_OK;
 }
 
+int layernorm_post_f16(cb_ctx* ctx, float* h, const float* gamma, const float* beta, void* y, int rows, int d, float eps, cudaStream_t stream) {
+  if (!h || !gamma || !beta || !y) return fail(ctx, CB_ERR_ARG, "layernorm_post: null operand");
+  if (rows < 0) return fail(ctx, CB_ERR_ARG, "layernorm_post: rows=%d", rows);
+  if (d <= 0 || d % 128 || d > 128 * kLnMaxChunks) return fail(ctx, CB_ERR_UNSUPPORTED, "layernorm_post: d=%d must be a multiple of 128 and <= %d", d, 128 * kLnMaxChunks);
+  if (rows == 0) return CB_OK;
+  mark_launch(ctx, CB_PROF_LAYERNORM, stream);
+  const unsigned grid = (unsigned)((rows + 7) / 8);
+  if (d >> 7 == 8)  // BERT-large, 1024
+    layernorm_post_kernel<8, 3><<<grid, 256, 0, stream>>>(h, gamma, beta, (__half*)y, rows, d, eps);
+  else
+    layernorm_post_kernel<0, 3><<<grid, 256, 0, stream>>>(h, gamma, beta, (__half*)y, rows, d, eps);
+  CB_CUDA(ctx, cudaGetLastError());
+  return CB_OK;
+}
+
 int assemble_tokens(cb_ctx* ctx, const float* patch, const float* cls, const float* pos, const float* gamma, const float* beta, float* h, int n,
                     int tokens, int grid2, int d, float eps, cudaStream_t stream) {
   if (d % 128 || d > 128 * kLnMaxChunks) return fail(ctx, CB_ERR_UNSUPPORTED, "assemble: d=%d unsupported", d);
@@ -744,6 +790,23 @@ int attention_f16(cb_ctx* ctx, const void* qkv, void* out, int n, int tokens, in
   else if (!stream_keys) CB_ATTN_LAUNCH(80, false);
   else CB_ATTN_LAUNCH(80, true);
 #undef CB_ATTN_LAUNCH
+  CB_CUDA(ctx, cudaGetLastError());
+  return CB_OK;
+}
+
+// The resident mma.sync kernel with per-image lengths (head_dim 64, tokens <= the resident limit, 352); other shapes: CB_ERR_UNSUPPORTED.
+int attention_masked_f16(cb_ctx* ctx, const void* qkv, void* out, int n, int tokens, int heads, int head_dim, const int* lengths, cudaStream_t stream) {
+  if (!qkv || !out || !lengths) return fail(ctx, CB_ERR_ARG, "attention_masked: null operand");
+  if (n < 0) return fail(ctx, CB_ERR_ARG, "attention_masked: n=%d", n);
+  if (n == 0) return CB_OK;
+  const int t_pad = (tokens + 15) & ~15;
+  const size_t smem = (size_t)2 * t_pad * (64 + 8) * 2;
+  if (head_dim != 64 || heads <= 0 || tokens <= 0 || smem > 100 * 1024)
+    return fail(ctx, CB_ERR_UNSUPPORTED, "attention_masked: tokens=%d heads=%d head_dim=%d unsupported (head_dim 64, tokens <= 352)", tokens, heads, head_dim);
+  mark_launch(ctx, CB_PROF_ATTENTION, stream);
+  CB_CUDA(ctx, cudaFuncSetAttribute(attention_kernel<64, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  attention_kernel<64, false, true><<<n * heads, kAttnThreads, smem, stream>>>((const __half*)qkv, (__half*)out, tokens, heads, head_dim,
+                                                                              1.4426950408889634f / sqrtf((float)head_dim), lengths);
   CB_CUDA(ctx, cudaGetLastError());
   return CB_OK;
 }
@@ -860,5 +923,13 @@ int cb_layernorm_f16(cb_ctx* ctx, const float* x, const float* gamma, const floa
 int cb_attention_f16(cb_ctx* ctx, const void* qkv, void* out, int n, int tokens, int heads, int head_dim, void* stream) {
   if (!ctx) return CB_ERR_ARG;
   return cb::attention_f16(ctx, qkv, out, n, tokens, heads, head_dim, (cudaStream_t)stream);
+}
+int cb_attention_masked_f16(cb_ctx* ctx, const void* qkv, void* out, int n, int tokens, int heads, int head_dim, const int* lengths, void* stream) {
+  if (!ctx) return CB_ERR_ARG;
+  return cb::attention_masked_f16(ctx, qkv, out, n, tokens, heads, head_dim, lengths, (cudaStream_t)stream);
+}
+int cb_layernorm_post_f16(cb_ctx* ctx, float* h, const float* gamma, const float* beta, void* y, int rows, int d, float eps, void* stream) {
+  if (!ctx) return CB_ERR_ARG;
+  return cb::layernorm_post_f16(ctx, h, gamma, beta, y, rows, d, eps, (cudaStream_t)stream);
 }
 }

@@ -100,6 +100,7 @@ except Exception:  # noqa: BLE001
         cosmos_embed1_embedding: np.ndarray | None = None
         intern_video_2_frames: LazyData = attrs.field(factory=LazyData, converter=LazyData.coerce)
         intern_video_2_embedding: np.ndarray | None = None
+        intern_video_2_text_match: tuple[str, float] | None = None
         openai_embedding: np.ndarray | None = None
         errors: dict[str, str] = attrs.Factory(dict)
 

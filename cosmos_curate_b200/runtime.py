@@ -13,7 +13,7 @@ import numpy as np
 import torch
 
 from . import _lib
-from ._lib import Iv2Cfg, SurfacePool, VitCfg, check
+from ._lib import Iv2Cfg, Iv2TextCfg, SurfacePool, VitCfg, check
 
 try:
     from loguru import logger
@@ -268,6 +268,33 @@ class Context(_Handle):
         check(self.lib.cb_attention_f16(self.h, qkv.data_ptr(), out.data_ptr(), n, t, heads, d // heads, _stream_ptr()), "cb_attention_f16", self.h)
         return out
 
+    def attention_masked(self, qkv: torch.Tensor, heads: int, lengths: torch.Tensor) -> torch.Tensor:
+        """cb_attention_masked_f16: sequence i of qkv [n][T][3 * hidden] attends to its first lengths[i] keys (int32 cuda [n])."""
+        n, t, three_d = qkv.shape
+        d = three_d // 3
+        assert lengths.is_cuda and lengths.dtype == torch.int32 and lengths.shape == (n,)
+        out = torch.empty((n, t, d), dtype=torch.float16, device=qkv.device)
+        check(self.lib.cb_attention_masked_f16(self.h, qkv.data_ptr(), out.data_ptr(), n, t, heads, d // heads, lengths.data_ptr(), _stream_ptr()),
+              "cb_attention_masked_f16", self.h)  # fmt: skip
+        return out
+
+    def layernorm_post_(self, h: torch.Tensor, gamma: torch.Tensor, beta: torch.Tensor, eps: float) -> torch.Tensor:
+        """cb_layernorm_post_f16: h (fp32 [rows][d]) normalised in place; returns the fp16 copy."""
+        rows, d = h.shape
+        y = torch.empty((rows, d), dtype=torch.float16, device=h.device)
+        check(self.lib.cb_layernorm_post_f16(self.h, h.data_ptr(), gamma.data_ptr(), beta.data_ptr(), y.data_ptr(), rows, d, eps, _stream_ptr()),
+              "cb_layernorm_post_f16", self.h)  # fmt: skip
+        return y
+
+    def text_embed(self, ids: torch.Tensor, word: torch.Tensor, pos: torch.Tensor, type_row: torch.Tensor) -> torch.Tensor:
+        """cb_text_embed: int32 cuda ids [n][L] -> fp32 (word[id] + type) + pos[t], [n][L][d]."""
+        n, L = ids.shape
+        d = word.shape[1]
+        h = torch.empty((n, L, d), dtype=torch.float32, device=ids.device)
+        check(self.lib.cb_text_embed(self.h, ids.data_ptr(), word.data_ptr(), pos.data_ptr(), type_row.data_ptr(), h.data_ptr(), n, L, d,
+                                     _stream_ptr()), "cb_text_embed", self.h)  # fmt: skip
+        return h
+
 
 _CONTEXTS: dict[int, Context] = {}
 
@@ -373,6 +400,40 @@ class Iv2Tower(_Handle):
         tubes = tubes.contiguous()
         out = torch.empty((tubes.shape[0], self.embed_dim), dtype=torch.float32, device=tubes.device)
         check(self.lib.cb_iv2_forward(self.h, tubes.data_ptr(), tubes.shape[0], out.data_ptr(), _stream_ptr()), "cb_iv2_forward", self.ctx.h)
+        return out
+
+
+class Iv2TextTower(_Handle):
+    """cb_iv2_text_* wrapper: weights in (fp32 numpy, names of include/curate_b200.h cb_iv2_text_set_tensor), text embeddings out."""
+
+    FIELDS = ("hidden", "layers", "heads", "mlp", "vocab", "max_pos", "embed_dim", "ln_eps")
+
+    def __init__(self, ctx: Context, cfg: dict, weights: dict, max_texts: int = 64, max_len: int = 40):
+        self.ctx, self.lib = ctx, ctx.lib
+        self.cfg = {k: cfg[k] for k in self.FIELDS}
+        h = C.c_void_p()
+        check(self.lib.cb_iv2_text_create(ctx.h, C.byref(Iv2TextCfg(*[self.cfg[k] for k in self.FIELDS])), C.byref(h)), "cb_iv2_text_create", ctx.h)
+        self.h = h
+        ctx._children.add(self)
+        for name, arr in weights.items():
+            a = np.ascontiguousarray(arr, dtype=np.float32)
+            check(self.lib.cb_iv2_text_set_tensor(self.h, name.encode(), a.ctypes.data_as(C.POINTER(C.c_float)), a.size),
+                  f"cb_iv2_text_set_tensor({name})", ctx.h)  # fmt: skip
+        check(self.lib.cb_iv2_text_finalize(self.h, max_texts, max_len), "cb_iv2_text_finalize", ctx.h)
+        self.embed_dim, self.max_texts, self.max_len = self.cfg["embed_dim"], max_texts, max_len
+
+    def _destroy(self):
+        self.lib.cb_iv2_text_destroy(self.h)
+
+    def forward(self, ids: np.ndarray, lengths: np.ndarray) -> torch.Tensor:
+        """Host int32 ids [n, L] and lengths [n] -> unit-norm float32 cuda [n, embed_dim]."""
+        ids = np.ascontiguousarray(ids, dtype=np.int32)
+        lengths = np.ascontiguousarray(lengths, dtype=np.int32)
+        assert ids.ndim == 2 and lengths.shape == (ids.shape[0],), (ids.shape, lengths.shape)
+        n, L = ids.shape
+        out = torch.empty((n, self.embed_dim), dtype=torch.float32, device=f"cuda:{self.ctx.device}")
+        check(self.lib.cb_iv2_text_forward(self.h, ids.ctypes.data_as(C.POINTER(C.c_int32)), lengths.ctypes.data_as(C.POINTER(C.c_int32)), n, L,
+                                           out.data_ptr(), _stream_ptr()), "cb_iv2_text_forward", self.ctx.h)  # fmt: skip
         return out
 
 

@@ -2,8 +2,11 @@
 (cosmos_curate/pipelines/video/embedding/internvideo2_stages.py:187-309): `clip.intern_video_2_embedding` <- float32 [1, 512] from
 the tube InternVideo2FrameCreationStage left in `clip.intern_video_2_frames`, which is dropped for every clip.
 
-Clips of all tasks of one call share the tower's batches (an embedding does not depend on its batch neighbours).  `texts_to_verify`
-needs the BERT text tower, which is not built: anything but None is refused at construction.  Build the pair as
+Clips of all tasks of one call share the tower's batches (an embedding does not depend on its batch neighbours).  With
+`texts_to_verify`, every clip whose embedding is set also gets `clip.intern_video_2_text_match = (text, probability)`: the most probable
+text under softmax(100 * clip . text) (_verify_with_texts, :251-256).  The texts are embedded once per stage, not once per clip as the
+reference does (a text's embedding does not depend on the clip).  An empty list, or a model that cannot embed text, is refused at
+construction.  Build the pair as
 InternVideo2FrameCreationStage(model=InternVideo2FrameFormulator(num_frames=4)) -> InternVideo2EmbeddingStage: a tube of another
 frame count raises ValueError naming both counts (the reference fails on the pos_embed add).
 """
@@ -20,16 +23,33 @@ class InternVideo2EmbeddingStage(CuratorStage):
 
     def __init__(self, num_gpus_per_worker: float = 0.25, batch_size: int = 8, *, verbose: bool = False, log_stats: bool = False,
                  texts_to_verify: list[str] | None = None, model: InternVideo2MultiModality | None = None) -> None:  # fmt: skip
+        self._model = model if model is not None else InternVideo2MultiModality()
         if texts_to_verify is not None:
-            msg = "texts_to_verify needs the InternVideo2 text tower (BERT), which this path does not build"
-            raise ValueError(msg)
+            if not texts_to_verify:
+                msg = "texts_to_verify is empty: give at least one text, or None"
+                raise ValueError(msg)
+            if not (callable(getattr(self._model, "encode_texts", None)) and callable(getattr(self._model, "evaluate", None))):
+                msg = f"texts_to_verify needs a model that embeds text (encode_texts / evaluate); {type(self._model).__name__} does not"
+                raise ValueError(msg)
+        self._texts = list(texts_to_verify) if texts_to_verify is not None else None
+        self._text_embeddings = None
         self._timer = StageTimer(self)
         self._num_gpus_per_worker, self._batch_size = num_gpus_per_worker, batch_size
         self._verbose, self._log_stats = verbose, log_stats
-        self._model = model if model is not None else InternVideo2MultiModality()
 
     def stage_setup(self) -> None:
         self._model.setup()
+        self._embed_texts()
+
+    def _embed_texts(self):
+        if self._texts is not None and self._text_embeddings is None:
+            self._text_embeddings = list(self._model.encode_texts(self._texts))
+        return self._text_embeddings
+
+    def _verify_with_texts(self, clip) -> None:
+        if self._texts is not None and clip.intern_video_2_embedding is not None:
+            probs, idxs = self._model.evaluate(clip.intern_video_2_embedding, self._embed_texts())
+            clip.intern_video_2_text_match = (self._texts[idxs[0]], probs[0])
 
     @property
     def model(self) -> ModelInterface:
@@ -59,6 +79,8 @@ class InternVideo2EmbeddingStage(CuratorStage):
                     assert len(embeddings) == len(todo), f"Expected {len(todo)} embeddings, but got {len(embeddings)}"
                     for clip, e in zip(todo, embeddings):
                         clip.intern_video_2_embedding = e
+                for clip in clips:
+                    self._verify_with_texts(clip)
             finally:
                 for clip in clips:
                     clip.intern_video_2_frames.drop()

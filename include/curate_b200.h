@@ -29,6 +29,7 @@ extern "C" {
 #define CB_ERR_NVDEC (-4)       /* libnvcuvid missing or decode failure */
 #define CB_ERR_DEMUX (-5)       /* malformed / unsupported container */
 #define CB_ERR_STATE (-6)       /* call order (e.g. forward before finalize) */
+#define CB_ERR_INVALID (-7)     /* input data out of range (e.g. a token id >= vocab, a text length outside [1, L]) */
 
 #define CB_ABI_VERSION 1
 
@@ -306,6 +307,20 @@ int cb_qk_rmsnorm_f16(cb_ctx* ctx, void* qkv, const float* q_weight, const float
  * cb_attention_f16 (qkv fp16 [n][tokens][3*hidden] -> out fp16 [n][tokens][hidden], scale head_dim^-1/2).  Any other head_dim:
  * CB_ERR_UNSUPPORTED.  n == 0 is a no-op. */
 int cb_attention_stream_f16(cb_ctx* ctx, const void* qkv, void* out, int n, int tokens, int heads, int head_dim, void* stream);
+/* cb_attention_f16 for sequences padded to `tokens`: lengths is device int32 [n], and image i attends only to its keys < lengths[i]
+ * (a BERT padding mask).  Keys and values past the length are never read, so whatever the padded rows hold cannot reach the output;
+ * output rows past the length are zeros.  Image i's rows below its length are bitwise what the mma.sync kernel gives the unpadded
+ * sequence of lengths[i] tokens, so with every length == tokens the output equals cb_attention_f16's whenever cb_attention_f16 runs
+ * that kernel (outside 129..257 tokens, or always with CB_ATTN_KERNEL=mma).  Lengths outside [0, tokens] are clamped to it.
+ * head_dim 64 and tokens <= 352 (K and V resident in shared memory) only; other shapes: CB_ERR_UNSUPPORTED.  n == 0 is a no-op. */
+int cb_attention_masked_f16(cb_ctx* ctx, const void* qkv, void* out, int n, int tokens, int heads, int head_dim, const int* lengths, void* stream);
+/* Post-LN (BERT's LayerNorm(x + sublayer(x)) with the sum already in h): h[rows][d] fp32 = LayerNorm(h) * gamma + beta in place, and
+ * y[rows][d] fp16 = the same values rounded.  Statistics as cb_layernorm_f16.  d % 128 == 0, d <= 1536. */
+int cb_layernorm_post_f16(cb_ctx* ctx, float* h, const float* gamma, const float* beta, void* y, int rows, int d, float eps, void* stream);
+/* BERT embeddings before their LayerNorm (xbert.py BertEmbeddings, token type 0): h[i][t] = (word[ids[i][t]] + type) + pos[t], fp32.
+ * ids device int32 [n][L] (not range-checked here), word [vocab][d], pos [>= L][d], type [d].  d % 4 == 0. */
+int cb_text_embed(cb_ctx* ctx, const int32_t* ids, const float* word, const float* pos, const float* type, float* h, int n, int L, int d,
+                  void* stream);
 
 /* ---- InternVideo2 video tower (clip embeddings) ------------------------------------------------------ */
 /* The vision half of InternVideo2_Stage2.get_vid_feat (models/internvideo2_mm.py:203-217): PretrainInternVideo2.forward
@@ -330,6 +345,30 @@ int cb_iv2_finalize(cb_iv2* iv2, int max_clips);
 /* tubes: device fp32 [n][frames][3][image_size][image_size] (InternVideo2FrameCreationStage's tubes); emb_out: device fp32
  * [n][embed_dim], unit norm.  Clips are independent: an embedding does not depend on the other clips of the call. */
 int cb_iv2_forward(cb_iv2* iv2, const float* tubes, int n, float* emb_out, void* stream);
+
+/* ---- InternVideo2 text tower (text embeddings) ------------------------------------------------------- */
+/* InternVideo2_Stage2.get_txt_feat (models/internvideo2_mm.py:219-241) after tokenization: BertModel(mode="text") (bert/xbert.py), i.e.
+ * the first `layers` (fusion_layer = 19) post-LN self-attention layers of BERT-large, the [CLS] row, text_proj and the L2 norm.  A
+ * handle of its own: a caller that never embeds text never loads its weights. */
+typedef struct cb_iv2_text cb_iv2_text;
+typedef struct cb_iv2_text_cfg {
+  int hidden, layers, heads, mlp; /* 1024, 19, 16, 4096 (head_dim 64 only) */
+  int vocab, max_pos, embed_dim;  /* 30522, 512, text_proj output 512 */
+  float ln_eps;                   /* 1e-12 */
+} cb_iv2_text_cfg;
+int cb_iv2_text_create(cb_ctx* ctx, const cb_iv2_text_cfg* cfg, cb_iv2_text** out);
+void cb_iv2_text_destroy(cb_iv2_text* text);
+/* Upload one named tensor (host fp32, row-major, `count` elements).  Names: tok_emb[vocab][h], pos_emb[max_pos][h], type_emb[h] (token
+ * type 0), emb_ln_w, emb_ln_b, L<i>.{qkv_w[3h][h] (query | key | value), qkv_b[3h], proj_w[h][h], proj_b, ln1_w, ln1_b, fc1_w[mlp][h],
+ * fc1_b, fc2_w[h][mlp], fc2_b, ln2_w, ln2_b}, tproj_w[embed_dim][h], tproj_b.  GEMM weights are stored as fp16, the rest stays fp32. */
+int cb_iv2_text_set_tensor(cb_iv2_text* text, const char* name, const float* data, size_t count);
+/* Checks that every tensor arrived and sizes the workspace for calls of up to max_texts texts (more are run in chunks) of up to max_len
+ * tokens; max_len <= min(max_pos, 352), else CB_ERR_UNSUPPORTED. */
+int cb_iv2_text_finalize(cb_iv2_text* text, int max_texts, int max_len);
+/* ids: HOST int32 [n][L] token ids ([CLS] ... [SEP], padded), lengths: HOST int32 [n]; emb_out: device fp32 [n][embed_dim], unit norm.
+ * An id outside [0, vocab), a length outside [1, L] or L outside [1, max_pos] is CB_ERR_INVALID (nothing is launched); L > max_len is
+ * CB_ERR_ARG.  A text's embedding is bitwise independent of the other texts of the call, its place among them and L. */
+int cb_iv2_text_forward(cb_iv2_text* text, const int32_t* ids, const int32_t* lengths, int n, int L, float* emb_out, void* stream);
 
 #ifdef __cplusplus
 }
