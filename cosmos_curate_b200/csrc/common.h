@@ -88,5 +88,31 @@ void release_tc_plans(cb_ctx* ctx);
 int ensure_norm_lut(cb_ctx* ctx, const float mean[3], const float std_[3], cudaStream_t stream);
 // NV12 -> RGB -> bilinear out_w x out_h for ONE surface at `base` (used on NVDEC-mapped frames), u8 HWC into `out`.
 int bilinear_from_surface(cb_ctx* ctx, const void* base, int pitch, int luma_rows, int w, int h, int out_w, int out_h, uint8_t* out, cudaStream_t stream);
+int run_clip_preprocess(cb_ctx* ctx, const cb_surface_pool* pool, const int32_t* slots, int n, int res, int out_mode, int layout_patch,
+                        int k_pad, int dtype, const float mean[3], const float std_[3], void* out, cudaStream_t stream);
+
+// Tower ops (gemm.cu, vit_kernels.cu, attention_*.cu): fp16 operands, fp32 accumulation, launched on `stream`.
+int gemm_f16(cb_ctx* ctx, const void* A, const void* W, const float* bias, const float* residual, float* out_f32, void* out_f16, int M,
+             int N, int K, int epilogue, cudaStream_t stream);
+int gemm_f16_ex(cb_ctx* ctx, const void* A, const void* W, const float* bias, const float* gamma, const float* residual, float* out_f32,
+                void* out_f16, int M, int N, int K, int epilogue, cudaStream_t stream);
+int layernorm_f16(cb_ctx* ctx, const float* x, const float* gamma, const float* beta, void* y, int rows, int d, float eps, cudaStream_t stream);
+int layernorm_post_f16(cb_ctx* ctx, float* h, const float* gamma, const float* beta, void* y, int rows, int d, float eps, cudaStream_t stream);
+int rmsnorm_f16(cb_ctx* ctx, const float* x, const float* w, void* y, int rows, int d, float eps, cudaStream_t stream);
+int qk_rmsnorm_f16(cb_ctx* ctx, void* qkv, const float* wq, const float* wk, int rows, int d, float eps, cudaStream_t stream);
+int assemble_tokens(cb_ctx* ctx, const float* patch, const float* cls, const float* pos, const float* gamma, const float* beta, float* h, int n,
+                    int tokens, int grid2, int d, float eps, cudaStream_t stream);
+int attention_f16(cb_ctx* ctx, const void* qkv, void* out, int n, int tokens, int heads, int head_dim, cudaStream_t stream);
+int attention_wgmma(cb_ctx* ctx, const void* qkv, void* out, int n, int tokens, int heads, int head_dim, cudaStream_t stream, bool* launched);
+int attention_masked_f16(cb_ctx* ctx, const void* qkv, void* out, int n, int tokens, int heads, int head_dim, const int* lengths, cudaStream_t stream);
+int attention_stream_f16(cb_ctx* ctx, const void* qkv, void* out, int n, int tokens, int heads, int head_dim, cudaStream_t stream);
+int map_pool(cb_ctx* ctx, const void* kv, const float* q, void* out, int n, int tokens, int heads, int head_dim, cudaStream_t stream);
+int clip_tail(cb_ctx* ctx, const float* h, size_t img_stride, const float* gamma, const float* beta, const float* proj, int d, int proj_dim,
+              float eps, const float* aes_w, float aes_b, float* emb_out, float* feat_out, float* score_out, int n, cudaStream_t stream);
+int l2norm_score(cb_ctx* ctx, const float* feat, int d, const float* aes_w, float aes_b, float* emb, float* feat_out, float* score, int n,
+                 cudaStream_t stream);
+int tube_patches(cb_ctx* ctx, const float* tubes, void* out, int frames, int image_size, int patch, int k_pad, cudaStream_t stream);
+int token_mean(cb_ctx* ctx, const float* h, float* out, int n, int tokens, int d, cudaStream_t stream);
+int clip_pool(cb_ctx* ctx, const float* q, const void* k, const void* v, void* out, int n, int tokens, int heads, int head_dim, cudaStream_t stream);
 
 }  // namespace cb

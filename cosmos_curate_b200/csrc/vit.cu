@@ -5,41 +5,20 @@
 
 #include <cmath>
 #include <cstring>
-#include <map>
-#include <string>
 #include <vector>
 
-#include "common.h"
-
-namespace cb {
-int gemm_f16(cb_ctx*, const void*, const void*, const float*, const float*, float*, void*, int, int, int, int, cudaStream_t);
-int layernorm_f16(cb_ctx*, const float*, const float*, const float*, void*, int, int, float, cudaStream_t);
-int assemble_tokens(cb_ctx*, const float*, const float*, const float*, const float*, const float*, float*, int, int, int, int, float, cudaStream_t);
-int attention_f16(cb_ctx*, const void*, void*, int, int, int, int, cudaStream_t);
-int clip_tail(cb_ctx*, const float*, size_t, const float*, const float*, const float*, int, int, float, const float*, float, float*, float*,
-              float*, int, cudaStream_t);
-int map_pool(cb_ctx*, const void*, const float*, void*, int, int, int, int, cudaStream_t);
-int l2norm_score(cb_ctx*, const float*, int, const float*, float, float*, float*, float*, int, cudaStream_t);
-int run_clip_preprocess(cb_ctx*, const cb_surface_pool*, const int32_t*, int, int, int, int, int, int, const float*, const float*, void*,
-                        cudaStream_t);
-}  // namespace cb
-
-struct cb_tensor {
-  void* d = nullptr;
-  size_t count = 0;
-  bool half = false;
-};
+#include "tower.h"
 
 struct cb_vit {
   cb_ctx* ctx = nullptr;
   cb_vit_cfg cfg{};
   int grid = 0, tokens = 0, kp = 0, k_pad = 0, out_dim = 0;
-  std::map<std::string, cb_tensor> t;
+  cb::WeightStore w;
   float* aes_w = nullptr;
   float aes_b = 0.f;
   bool finalized = false;
   int max_batch = 0;
-  // workspace
+  cb::Workspace ws;
   float *patch_out = nullptr, *h = nullptr;
   __half *xn = nullptr, *qkv = nullptr, *attn = nullptr, *mlp = nullptr, *patches = nullptr;
   // SigLIP MAP head: the pooling query is image-independent -> q = (probe Wq^T + bq) / sqrt(head_dim), folded at finalize
@@ -49,50 +28,40 @@ struct cb_vit {
 
 namespace {
 
-struct Expect {
-  size_t count;
-  bool half;
-};
+enum Global { PATCH_W, PATCH_B, POS, CLS, PRE_LN_W, PRE_LN_B, POST_LN_W, POST_LN_B, PROJ_W, MAP_PROBE, MAP_IN_W, MAP_IN_B, MAP_OUT_W,
+              MAP_OUT_B, MAP_LN_W, MAP_LN_B, MAP_FC1_W, MAP_FC1_B, MAP_FC2_W, MAP_FC2_B, kGlobals };
+enum Leaf { LN1_W, LN1_B, QKV_W, QKV_B, OUT_W, OUT_B, LN2_W, LN2_B, FC1_W, FC1_B, FC2_W, FC2_B, kLeaves };
 
-std::map<std::string, Expect> expected_tensors(const cb_vit* v) {
+void declare_tensors(cb_vit* v) {
+  using cb::F16;
   const cb_vit_cfg& c = v->cfg;
   const size_t d = c.hidden, m = c.mlp;
-  std::map<std::string, Expect> e;
-  e["patch_w"] = {d * (size_t)v->kp, true};
-  e["pos"] = {(size_t)v->tokens * d, false};
+  cb::WeightStore& w = v->w;
+  w.layout(kGlobals, kLeaves, c.layers);
+  w.add(PATCH_W, "patch_w", d * v->kp, F16, v->kp, v->k_pad);
+  w.add(POS, "pos", (size_t)v->tokens * d);
   if (c.arch == CB_ARCH_CLIP) {
-    e["cls"] = {d, false};
-    e["pre_ln_w"] = {d, false};
-    e["pre_ln_b"] = {d, false};
+    w.add(CLS, "cls", d);
+    w.add(PRE_LN_W, "pre_ln_w", d), w.add(PRE_LN_B, "pre_ln_b", d);
   } else {
-    e["patch_b"] = {d, false};
+    w.add(PATCH_B, "patch_b", d);
   }
-  for (int i = 0; i < c.layers; ++i) {
-    const std::string p = "L" + std::to_string(i) + ".";
-    e[p + "ln1_w"] = {d, false}, e[p + "ln1_b"] = {d, false};
-    e[p + "qkv_w"] = {3 * d * d, true}, e[p + "qkv_b"] = {3 * d, false};
-    e[p + "out_w"] = {d * d, true}, e[p + "out_b"] = {d, false};
-    e[p + "ln2_w"] = {d, false}, e[p + "ln2_b"] = {d, false};
-    e[p + "fc1_w"] = {m * d, true}, e[p + "fc1_b"] = {m, false};
-    e[p + "fc2_w"] = {d * m, true}, e[p + "fc2_b"] = {d, false};
-  }
-  e["post_ln_w"] = {d, false}, e["post_ln_b"] = {d, false};
-  if (c.proj_dim > 0) e["proj_w"] = {(size_t)c.proj_dim * d, false};
+  w.add_leaf(LN1_W, "ln1_w", d), w.add_leaf(LN1_B, "ln1_b", d);
+  w.add_leaf(QKV_W, "qkv_w", 3 * d * d, F16), w.add_leaf(QKV_B, "qkv_b", 3 * d);
+  w.add_leaf(OUT_W, "out_w", d * d, F16), w.add_leaf(OUT_B, "out_b", d);
+  w.add_leaf(LN2_W, "ln2_w", d), w.add_leaf(LN2_B, "ln2_b", d);
+  w.add_leaf(FC1_W, "fc1_w", m * d, F16), w.add_leaf(FC1_B, "fc1_b", m);
+  w.add_leaf(FC2_W, "fc2_w", d * m, F16), w.add_leaf(FC2_B, "fc2_b", d);
+  w.add(POST_LN_W, "post_ln_w", d), w.add(POST_LN_B, "post_ln_b", d);
+  if (c.proj_dim > 0) w.add(PROJ_W, "proj_w", (size_t)c.proj_dim * d);
   if (c.arch == CB_ARCH_SIGLIP) {
-    e["map_probe"] = {d, false};
-    e["map_in_w"] = {3 * d * d, true}, e["map_in_b"] = {3 * d, false};
-    e["map_out_w"] = {d * d, true}, e["map_out_b"] = {d, false};
-    e["map_ln_w"] = {d, false}, e["map_ln_b"] = {d, false};
-    e["map_fc1_w"] = {m * d, true}, e["map_fc1_b"] = {m, false};
-    e["map_fc2_w"] = {d * m, true}, e["map_fc2_b"] = {d, false};
+    w.add(MAP_PROBE, "map_probe", d);
+    w.add(MAP_IN_W, "map_in_w", 3 * d * d, F16), w.add(MAP_IN_B, "map_in_b", 3 * d);
+    w.add(MAP_OUT_W, "map_out_w", d * d, F16), w.add(MAP_OUT_B, "map_out_b", d);
+    w.add(MAP_LN_W, "map_ln_w", d), w.add(MAP_LN_B, "map_ln_b", d);
+    w.add(MAP_FC1_W, "map_fc1_w", m * d, F16), w.add(MAP_FC1_B, "map_fc1_b", m);
+    w.add(MAP_FC2_W, "map_fc2_w", d * m, F16), w.add(MAP_FC2_B, "map_fc2_b", d);
   }
-  return e;
-}
-
-template <typename T>
-int dev_alloc(cb_ctx* ctx, T** p, size_t count) {
-  CB_CUDA(ctx, cudaMalloc((void**)p, count * sizeof(T)));
-  return CB_OK;
 }
 
 }  // namespace
@@ -121,6 +90,7 @@ int cb_vit_create(cb_ctx* ctx, const cb_vit_cfg* cfg, cb_vit** out) {
   v->kp = 3 * c.patch * c.patch;
   v->k_pad = (v->kp + 63) & ~63;
   v->out_dim = c.proj_dim > 0 ? c.proj_dim : c.hidden;
+  declare_tensors(v);
   *out = v;
   return CB_OK;
 }
@@ -128,10 +98,7 @@ int cb_vit_create(cb_ctx* ctx, const cb_vit_cfg* cfg, cb_vit** out) {
 void cb_vit_destroy(cb_vit* v) {
   if (!v) return;
   cudaSetDevice(v->ctx->device);
-  for (auto& kv : v->t) cudaFree(kv.second.d);
   cudaFree(v->aes_w);
-  cudaFree(v->map_q);
-  cudaFree(v->patch_out), cudaFree(v->h), cudaFree(v->xn), cudaFree(v->qkv), cudaFree(v->attn), cudaFree(v->mlp), cudaFree(v->patches);
   delete v;
 }
 
@@ -139,36 +106,13 @@ int cb_vit_k_pad(const cb_vit* v) { return v ? v->k_pad : CB_ERR_ARG; }
 
 int cb_vit_set_tensor(cb_vit* v, const char* name, const float* data, size_t count) {
   if (!v) return CB_ERR_ARG;
-  cb_ctx* ctx = v->ctx;
-  if (!name || !data) return cb::fail(ctx, CB_ERR_ARG, "vit_set_tensor: null argument");
-  auto exp = expected_tensors(v);
-  auto it = exp.find(name);
-  if (it == exp.end()) return cb::fail(ctx, CB_ERR_ARG, "vit_set_tensor: unknown tensor '%s'", name);
-  if (it->second.count != count) return cb::fail(ctx, CB_ERR_ARG, "vit_set_tensor: '%s' has %zu elements, expected %zu", name, count, it->second.count);
+  v->finalized = false;
+  if (const int rc = v->w.set(v->ctx, "vit", name, data, count)) return rc;
   // host copies of the pieces the MAP query is folded from
   const size_t dd = (size_t)v->cfg.hidden;
   if (std::strcmp(name, "map_probe") == 0) v->h_probe.assign(data, data + count);
   if (std::strcmp(name, "map_in_w") == 0) v->h_wq.assign(data, data + dd * dd);
   if (std::strcmp(name, "map_in_b") == 0) v->h_bq.assign(data, data + dd);
-  cb_tensor& t = v->t[name];
-  if (t.d) cudaFree(t.d), t.d = nullptr;
-  t.half = it->second.half;
-  if (!t.half) {
-    t.count = count;
-    CB_CUDA(ctx, cudaMalloc(&t.d, count * sizeof(float)));
-    CB_CUDA(ctx, cudaMemcpy(t.d, data, count * sizeof(float), cudaMemcpyHostToDevice));
-    return CB_OK;
-  }
-  // GEMM weights: fp32 -> fp16 (round to nearest even) on the host; patch_w rows zero-padded to k_pad
-  const bool is_patch = std::strcmp(name, "patch_w") == 0;
-  const size_t rows = is_patch ? (size_t)v->cfg.hidden : 1, in_cols = is_patch ? (size_t)v->kp : count;
-  const size_t out_cols = is_patch ? (size_t)v->k_pad : count;
-  std::vector<__half> hbuf(rows * out_cols, __float2half_rn(0.f));
-  for (size_t r = 0; r < rows; ++r)
-    for (size_t c2 = 0; c2 < in_cols; ++c2) hbuf[r * out_cols + c2] = __float2half_rn(data[r * in_cols + c2]);
-  t.count = hbuf.size();
-  CB_CUDA(ctx, cudaMalloc(&t.d, hbuf.size() * sizeof(__half)));
-  CB_CUDA(ctx, cudaMemcpy(t.d, hbuf.data(), hbuf.size() * sizeof(__half), cudaMemcpyHostToDevice));
   return CB_OK;
 }
 
@@ -186,22 +130,20 @@ int cb_vit_finalize(cb_vit* v, int max_batch) {
   if (!v) return CB_ERR_ARG;
   cb_ctx* ctx = v->ctx;
   if (max_batch <= 0) return cb::fail(ctx, CB_ERR_ARG, "vit_finalize: max_batch must be positive");
-  for (auto& kv : expected_tensors(v))
-    if (!v->t.count(kv.first)) return cb::fail(ctx, CB_ERR_STATE, "vit_finalize: tensor '%s' was never set", kv.first.c_str());
+  int rc;
+  if ((rc = v->w.check_complete(ctx, "vit_finalize"))) return rc;
   const cb_vit_cfg& c = v->cfg;
   const size_t rows = (size_t)max_batch * v->tokens, prow = (size_t)max_batch * v->grid * v->grid, d = c.hidden;
-  if (v->finalized) {
-    cudaFree(v->patch_out), cudaFree(v->h), cudaFree(v->xn), cudaFree(v->qkv), cudaFree(v->attn), cudaFree(v->mlp), cudaFree(v->patches);
-    v->finalized = false;
-  }
-  int rc;
-  if ((rc = dev_alloc(ctx, &v->patch_out, prow * d))) return rc;
-  if ((rc = dev_alloc(ctx, &v->h, rows * d))) return rc;
-  if ((rc = dev_alloc(ctx, &v->xn, rows * d))) return rc;
-  if ((rc = dev_alloc(ctx, &v->qkv, rows * 3 * d))) return rc;
-  if ((rc = dev_alloc(ctx, &v->attn, rows * d))) return rc;
-  if ((rc = dev_alloc(ctx, &v->mlp, rows * (size_t)c.mlp))) return rc;
-  if ((rc = dev_alloc(ctx, &v->patches, prow * (size_t)v->k_pad))) return rc;
+  cb::Workspace& ws = v->ws;
+  v->finalized = false;
+  ws.release();
+  if ((rc = ws.alloc(ctx, &v->patch_out, prow * d))) return rc;
+  if ((rc = ws.alloc(ctx, &v->h, rows * d))) return rc;
+  if ((rc = ws.alloc(ctx, &v->xn, rows * d))) return rc;
+  if ((rc = ws.alloc(ctx, &v->qkv, rows * 3 * d))) return rc;
+  if ((rc = ws.alloc(ctx, &v->attn, rows * d))) return rc;
+  if ((rc = ws.alloc(ctx, &v->mlp, rows * (size_t)c.mlp))) return rc;
+  if ((rc = ws.alloc(ctx, &v->patches, prow * (size_t)v->k_pad))) return rc;
   if (c.arch == CB_ARCH_SIGLIP) {
     const int dm = c.hidden, hd = dm / c.heads;
     std::vector<float> q(dm);
@@ -211,7 +153,7 @@ int cb_vit_finalize(cb_vit* v, int max_batch) {
       for (int i = 0; i < dm; ++i) acc += (double)v->h_wq[(size_t)o * dm + i] * (double)v->h_probe[i];
       q[o] = (float)(acc * sc);
     }
-    if (!v->map_q && (rc = dev_alloc(ctx, &v->map_q, (size_t)dm))) return rc;
+    if ((rc = ws.alloc(ctx, &v->map_q, (size_t)dm))) return rc;
     CB_CUDA(ctx, cudaMemcpy(v->map_q, q.data(), dm * sizeof(float), cudaMemcpyHostToDevice));
   }
   v->max_batch = max_batch;
@@ -222,43 +164,41 @@ int cb_vit_finalize(cb_vit* v, int max_batch) {
 static int forward_chunk(cb_vit* v, const void* patches, int n, float* emb, float* feat, float* score, cudaStream_t s) {
   cb_ctx* ctx = v->ctx;
   const cb_vit_cfg& c = v->cfg;
+  const cb::WeightStore& w = v->w;
   const int d = c.hidden, T = v->tokens, g2 = v->grid * v->grid, rows = n * T, hd = d / c.heads;
-  auto F = [&](const std::string& k) { return (const float*)v->t[k].d; };
-  auto H = [&](const std::string& k) { return (const void*)v->t[k].d; };
   const int act = c.act == CB_ACT_QUICK_GELU ? CB_EPI_QUICK_GELU : CB_EPI_GELU_TANH;
   int rc;
   // patch embedding (Conv2d stride=kernel=patch as a GEMM over im2col rows), fp32 out
-  if ((rc = cb::gemm_f16(ctx, patches, H("patch_w"), c.arch == CB_ARCH_SIGLIP ? F("patch_b") : nullptr, nullptr, v->patch_out, nullptr, n * g2, d,
+  if ((rc = cb::gemm_f16(ctx, patches, w.h(PATCH_W), c.arch == CB_ARCH_SIGLIP ? w.f(PATCH_B) : nullptr, nullptr, v->patch_out, nullptr, n * g2, d,
                          v->k_pad, CB_EPI_NONE, s)))
     return rc;
   if (c.arch == CB_ARCH_CLIP)
-    rc = cb::assemble_tokens(ctx, v->patch_out, F("cls"), F("pos"), F("pre_ln_w"), F("pre_ln_b"), v->h, n, T, g2, d, c.ln_eps, s);
+    rc = cb::assemble_tokens(ctx, v->patch_out, w.f(CLS), w.f(POS), w.f(PRE_LN_W), w.f(PRE_LN_B), v->h, n, T, g2, d, c.ln_eps, s);
   else
-    rc = cb::assemble_tokens(ctx, v->patch_out, nullptr, F("pos"), nullptr, nullptr, v->h, n, T, g2, d, c.ln_eps, s);
+    rc = cb::assemble_tokens(ctx, v->patch_out, nullptr, w.f(POS), nullptr, nullptr, v->h, n, T, g2, d, c.ln_eps, s);
   if (rc) return rc;
   for (int i = 0; i < c.layers; ++i) {
-    const std::string p = "L" + std::to_string(i) + ".";
-    if ((rc = cb::layernorm_f16(ctx, v->h, F(p + "ln1_w"), F(p + "ln1_b"), v->xn, rows, d, c.ln_eps, s))) return rc;
-    if ((rc = cb::gemm_f16(ctx, v->xn, H(p + "qkv_w"), F(p + "qkv_b"), nullptr, nullptr, v->qkv, rows, 3 * d, d, CB_EPI_NONE, s))) return rc;
+    if ((rc = cb::layernorm_f16(ctx, v->h, w.f(i, LN1_W), w.f(i, LN1_B), v->xn, rows, d, c.ln_eps, s))) return rc;
+    if ((rc = cb::gemm_f16(ctx, v->xn, w.h(i, QKV_W), w.f(i, QKV_B), nullptr, nullptr, v->qkv, rows, 3 * d, d, CB_EPI_NONE, s))) return rc;
     if ((rc = cb::attention_f16(ctx, v->qkv, v->attn, n, T, c.heads, hd, s))) return rc;
-    if ((rc = cb::gemm_f16(ctx, v->attn, H(p + "out_w"), F(p + "out_b"), v->h, v->h, nullptr, rows, d, d, CB_EPI_NONE, s))) return rc;
-    if ((rc = cb::layernorm_f16(ctx, v->h, F(p + "ln2_w"), F(p + "ln2_b"), v->xn, rows, d, c.ln_eps, s))) return rc;
-    if ((rc = cb::gemm_f16(ctx, v->xn, H(p + "fc1_w"), F(p + "fc1_b"), nullptr, nullptr, v->mlp, rows, c.mlp, d, act, s))) return rc;
-    if ((rc = cb::gemm_f16(ctx, v->mlp, H(p + "fc2_w"), F(p + "fc2_b"), v->h, v->h, nullptr, rows, d, c.mlp, CB_EPI_NONE, s))) return rc;
+    if ((rc = cb::gemm_f16(ctx, v->attn, w.h(i, OUT_W), w.f(i, OUT_B), v->h, v->h, nullptr, rows, d, d, CB_EPI_NONE, s))) return rc;
+    if ((rc = cb::layernorm_f16(ctx, v->h, w.f(i, LN2_W), w.f(i, LN2_B), v->xn, rows, d, c.ln_eps, s))) return rc;
+    if ((rc = cb::gemm_f16(ctx, v->xn, w.h(i, FC1_W), w.f(i, FC1_B), nullptr, nullptr, v->mlp, rows, c.mlp, d, act, s))) return rc;
+    if ((rc = cb::gemm_f16(ctx, v->mlp, w.h(i, FC2_W), w.f(i, FC2_B), v->h, v->h, nullptr, rows, d, c.mlp, CB_EPI_NONE, s))) return rc;
   }
   if (c.arch == CB_ARCH_CLIP)
-    return cb::clip_tail(ctx, v->h, (size_t)T * d, F("post_ln_w"), F("post_ln_b"), c.proj_dim > 0 ? F("proj_w") : nullptr, d, c.proj_dim, c.ln_eps,
+    return cb::clip_tail(ctx, v->h, (size_t)T * d, w.f(POST_LN_W), w.f(POST_LN_B), c.proj_dim > 0 ? w.f(PROJ_W) : nullptr, d, c.proj_dim, c.ln_eps,
                          score ? v->aes_w : nullptr, v->aes_b, emb, feat, score, n, s);
   // SigLIP: post_layernorm on every token, then the MAP head (one learned query attends over the tokens, + MLP block)
-  const __half* kv_w = (const __half*)H("map_in_w") + (size_t)d * d;  // rows d..3d of in_proj_weight: K | V projections
-  float* r = v->patch_out;                                            // [n][d] fp32 scratch (patch-embed output is dead by now)
-  if ((rc = cb::layernorm_f16(ctx, v->h, F("post_ln_w"), F("post_ln_b"), v->xn, rows, d, c.ln_eps, s))) return rc;
-  if ((rc = cb::gemm_f16(ctx, v->xn, kv_w, F("map_in_b") + d, nullptr, nullptr, v->qkv, rows, 2 * d, d, CB_EPI_NONE, s))) return rc;
+  const __half* kv_w = (const __half*)w.h(MAP_IN_W) + (size_t)d * d;  // rows d..3d of in_proj_weight: K | V projections
+  float* r = v->patch_out;                                             // [n][d] fp32 scratch (patch-embed output is dead by now)
+  if ((rc = cb::layernorm_f16(ctx, v->h, w.f(POST_LN_W), w.f(POST_LN_B), v->xn, rows, d, c.ln_eps, s))) return rc;
+  if ((rc = cb::gemm_f16(ctx, v->xn, kv_w, w.f(MAP_IN_B) + d, nullptr, nullptr, v->qkv, rows, 2 * d, d, CB_EPI_NONE, s))) return rc;
   if ((rc = cb::map_pool(ctx, v->qkv, v->map_q, v->attn, n, T, c.heads, hd, s))) return rc;
-  if ((rc = cb::gemm_f16(ctx, v->attn, H("map_out_w"), F("map_out_b"), nullptr, r, nullptr, n, d, d, CB_EPI_NONE, s))) return rc;
-  if ((rc = cb::layernorm_f16(ctx, r, F("map_ln_w"), F("map_ln_b"), v->xn, n, d, c.ln_eps, s))) return rc;
-  if ((rc = cb::gemm_f16(ctx, v->xn, H("map_fc1_w"), F("map_fc1_b"), nullptr, nullptr, v->mlp, n, c.mlp, d, act, s))) return rc;
-  if ((rc = cb::gemm_f16(ctx, v->mlp, H("map_fc2_w"), F("map_fc2_b"), r, r, nullptr, n, d, c.mlp, CB_EPI_NONE, s))) return rc;
+  if ((rc = cb::gemm_f16(ctx, v->attn, w.h(MAP_OUT_W), w.f(MAP_OUT_B), nullptr, r, nullptr, n, d, d, CB_EPI_NONE, s))) return rc;
+  if ((rc = cb::layernorm_f16(ctx, r, w.f(MAP_LN_W), w.f(MAP_LN_B), v->xn, n, d, c.ln_eps, s))) return rc;
+  if ((rc = cb::gemm_f16(ctx, v->xn, w.h(MAP_FC1_W), w.f(MAP_FC1_B), nullptr, nullptr, v->mlp, n, c.mlp, d, act, s))) return rc;
+  if ((rc = cb::gemm_f16(ctx, v->mlp, w.h(MAP_FC2_W), w.f(MAP_FC2_B), r, r, nullptr, n, d, c.mlp, CB_EPI_NONE, s))) return rc;
   return cb::l2norm_score(ctx, r, d, score ? v->aes_w : nullptr, v->aes_b, emb, feat, score, n, s);
 }
 
@@ -269,13 +209,10 @@ int cb_vit_forward(cb_vit* v, const void* patches, int n, float* emb_out, float*
   if (n < 0 || (n > 0 && (!patches || !emb_out))) return cb::fail(ctx, CB_ERR_ARG, "vit_forward: null argument");
   if (score_out && !v->aes_w) return cb::fail(ctx, CB_ERR_STATE, "vit_forward: scores requested but no aesthetic head was set");
   const size_t prow = (size_t)v->grid * v->grid * v->k_pad;
-  for (int i = 0; i < n; i += v->max_batch) {
-    const int m = std::min(v->max_batch, n - i);
-    int rc = forward_chunk(v, (const __half*)patches + (size_t)i * prow, m, emb_out + (size_t)i * v->out_dim,
-                           feat_out ? feat_out + (size_t)i * v->out_dim : nullptr, score_out ? score_out + i : nullptr, (cudaStream_t)stream);
-    if (rc) return rc;
-  }
-  return CB_OK;
+  return cb::for_chunks(n, v->max_batch, [&](int i, int m) {
+    return forward_chunk(v, (const __half*)patches + (size_t)i * prow, m, emb_out + (size_t)i * v->out_dim,
+                         feat_out ? feat_out + (size_t)i * v->out_dim : nullptr, score_out ? score_out + i : nullptr, (cudaStream_t)stream);
+  });
 }
 
 int cb_vit_embed_surfaces(cb_vit* v, const cb_surface_pool* pool, const int32_t* slots, int n, const float mean[3], const float std_[3],
@@ -285,16 +222,12 @@ int cb_vit_embed_surfaces(cb_vit* v, const cb_surface_pool* pool, const int32_t*
   if (!v->finalized) return cb::fail(ctx, CB_ERR_STATE, "vit_embed_surfaces before vit_finalize");
   if (n < 0 || (n > 0 && (!slots || !emb_out || !mean || !std_))) return cb::fail(ctx, CB_ERR_ARG, "vit_embed_surfaces: null argument");
   if (score_out && !v->aes_w) return cb::fail(ctx, CB_ERR_STATE, "vit_embed_surfaces: scores requested but no aesthetic head was set");
-  for (int i = 0; i < n; i += v->max_batch) {
-    const int m = std::min(v->max_batch, n - i);
-    int rc = cb::run_clip_preprocess(ctx, pool, slots + i, m, v->cfg.image_size, 2, v->cfg.patch, v->k_pad, CB_DT_F16, mean, std_, v->patches,
-                                     (cudaStream_t)stream);
-    if (rc) return rc;
-    rc = forward_chunk(v, v->patches, m, emb_out + (size_t)i * v->out_dim, feat_out ? feat_out + (size_t)i * v->out_dim : nullptr,
-                       score_out ? score_out + i : nullptr, (cudaStream_t)stream);
-    if (rc) return rc;
-  }
-  return CB_OK;
+  return cb::for_chunks(n, v->max_batch, [&](int i, int m) {
+    const int rc = cb::run_clip_preprocess(ctx, pool, slots + i, m, v->cfg.image_size, 2, v->cfg.patch, v->k_pad, CB_DT_F16, mean, std_, v->patches,
+                                           (cudaStream_t)stream);
+    return rc ? rc : forward_chunk(v, v->patches, m, emb_out + (size_t)i * v->out_dim, feat_out ? feat_out + (size_t)i * v->out_dim : nullptr,
+                                   score_out ? score_out + i : nullptr, (cudaStream_t)stream);
+  });
 }
 
 }  // extern "C"

@@ -760,8 +760,6 @@ int assemble_tokens(cb_ctx* ctx, const float* patch, const float* cls, const flo
   return CB_OK;
 }
 
-int attention_wgmma(cb_ctx* ctx, const void* qkv, void* out, int n, int tokens, int heads, int head_dim, cudaStream_t stream, bool* launched);
-
 int attention_f16(cb_ctx* ctx, const void* qkv, void* out, int n, int tokens, int heads, int head_dim, cudaStream_t stream) {
   if (!qkv || !out) return fail(ctx, CB_ERR_ARG, "attention: null operand");
   if (n <= 0) return CB_OK;

@@ -315,6 +315,13 @@ def affine_score(ctx: Context, emb: torch.Tensor, w: torch.Tensor, b: float) -> 
     return out
 
 
+def _set_tensors(ctx: Context, set_tensor, h, weights: dict) -> None:
+    """Upload every named array of `weights` as contiguous fp32 through `set_tensor`, one of the library's cb_*_set_tensor functions."""
+    for name, arr in weights.items():
+        a = np.ascontiguousarray(arr, dtype=np.float32)
+        check(set_tensor(h, name.encode(), a.ctypes.data_as(C.POINTER(C.c_float)), a.size), f"{set_tensor.__name__}({name})", ctx.h)
+
+
 class Pool:
     def __init__(self, buf: torch.Tensor, desc: SurfacePool):
         self.buf, self.desc = buf, desc  # keep the tensor alive while the descriptor is in use
@@ -333,9 +340,7 @@ class VitTower(_Handle):
         check(self.lib.cb_vit_create(ctx.h, C.byref(c), C.byref(h)), "cb_vit_create", ctx.h)
         self.h = h
         ctx._children.add(self)
-        for name, arr in weights.items():
-            a = np.ascontiguousarray(arr, dtype=np.float32)
-            check(self.lib.cb_vit_set_tensor(self.h, name.encode(), a.ctypes.data_as(C.POINTER(C.c_float)), a.size), f"cb_vit_set_tensor({name})", ctx.h)
+        _set_tensors(ctx, self.lib.cb_vit_set_tensor, self.h, weights)
         self.out_dim = cfg["proj_dim"] or cfg["hidden"]
         self.has_aesthetic = False
         if aesthetic is not None:
@@ -384,9 +389,7 @@ class Iv2Tower(_Handle):
         check(self.lib.cb_iv2_create(ctx.h, C.byref(Iv2Cfg(*[self.cfg[k] for k in self.FIELDS])), C.byref(h)), "cb_iv2_create", ctx.h)
         self.h = h
         ctx._children.add(self)
-        for name, arr in weights.items():
-            a = np.ascontiguousarray(arr, dtype=np.float32)
-            check(self.lib.cb_iv2_set_tensor(self.h, name.encode(), a.ctypes.data_as(C.POINTER(C.c_float)), a.size), f"cb_iv2_set_tensor({name})", ctx.h)
+        _set_tensors(ctx, self.lib.cb_iv2_set_tensor, self.h, weights)
         check(self.lib.cb_iv2_finalize(self.h, max_clips), "cb_iv2_finalize", ctx.h)
         self.frames, self.embed_dim, self.max_clips = self.cfg["frames"], self.cfg["embed_dim"], max_clips
 
@@ -415,10 +418,7 @@ class Iv2TextTower(_Handle):
         check(self.lib.cb_iv2_text_create(ctx.h, C.byref(Iv2TextCfg(*[self.cfg[k] for k in self.FIELDS])), C.byref(h)), "cb_iv2_text_create", ctx.h)
         self.h = h
         ctx._children.add(self)
-        for name, arr in weights.items():
-            a = np.ascontiguousarray(arr, dtype=np.float32)
-            check(self.lib.cb_iv2_text_set_tensor(self.h, name.encode(), a.ctypes.data_as(C.POINTER(C.c_float)), a.size),
-                  f"cb_iv2_text_set_tensor({name})", ctx.h)  # fmt: skip
+        _set_tensors(ctx, self.lib.cb_iv2_text_set_tensor, self.h, weights)
         check(self.lib.cb_iv2_text_finalize(self.h, max_texts, max_len), "cb_iv2_text_finalize", ctx.h)
         self.embed_dim, self.max_texts, self.max_len = self.cfg["embed_dim"], max_texts, max_len
 
@@ -448,11 +448,9 @@ class ShotNet(_Handle):
         check(self.lib.cb_transnet_create(ctx.h, C.byref(h)), "cb_transnet_create", ctx.h)
         self.h = h
         ctx._children.add(self)
-        for name, arr in state_dict.items():
-            if name in self.UNUSED_KEYS or name.endswith("num_batches_tracked"):
-                continue
-            a = np.ascontiguousarray(arr.detach().cpu().numpy() if isinstance(arr, torch.Tensor) else arr, dtype=np.float32)
-            check(self.lib.cb_transnet_set_tensor(self.h, name.encode(), a.ctypes.data_as(C.c_void_p), a.size), f"cb_transnet_set_tensor({name})", ctx.h)
+        weights = {name: arr.detach().cpu().numpy() if isinstance(arr, torch.Tensor) else arr for name, arr in state_dict.items()
+                   if name not in self.UNUSED_KEYS and not name.endswith("num_batches_tracked")}  # fmt: skip
+        _set_tensors(ctx, self.lib.cb_transnet_set_tensor, self.h, weights)
         check(self.lib.cb_transnet_finalize(self.h, max_windows), "cb_transnet_finalize", ctx.h)
         self.max_windows = max_windows
 

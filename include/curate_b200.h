@@ -153,7 +153,10 @@ int cb_vit_create(cb_ctx* ctx, const cb_vit_cfg* cfg, cb_vit** out);
 void cb_vit_destroy(cb_vit* vit);
 /* Upload one named tensor (host fp32, row-major, `count` elements).  Names: patch_w[hidden][3*p*p],
  * patch_b, cls, pos[tokens][hidden], pre_ln_w/b, L<i>.{ln1_w,ln1_b,qkv_w[3h][h],qkv_b,out_w,out_b,ln2_w,
- * ln2_b,fc1_w[mlp][h],fc1_b,fc2_w[h][mlp],fc2_b}, post_ln_w/b, proj_w[proj][hidden], map_* (SigLIP). */
+ * ln2_b,fc1_w[mlp][h],fc1_b,fc2_w[h][mlp],fc2_b}, post_ln_w/b, proj_w[proj][hidden], map_* (SigLIP).
+ * Tower handle lifecycle (cb_vit, cb_iv2, cb_iv2_text): set_tensor every tensor, then finalize, then forward.  A set_tensor call
+ * (replacing a tensor included) un-finalizes the handle: forward returns CB_ERR_STATE until the next finalize, which also re-derives
+ * what it folds from the weights (SigLIP's pooling query).  cb_vit_set_aesthetic writes in place and needs no new finalize. */
 int cb_vit_set_tensor(cb_vit* vit, const char* name, const float* data, size_t count);
 /* Aesthetic head folded to score = w . embedding + b (the reference MLP, aesthetics.py:44-53, has no
  * non-linearity).  w has proj_dim (or hidden) entries.  Optional. */
@@ -338,7 +341,7 @@ void cb_iv2_destroy(cb_iv2* iv2);
  * patch_b, cls, pos[tokens][hidden], L<i>.{norm1_w, qkv_w[3h][h], q_norm_w, k_norm_w, proj_w[h][h], proj_b, ls1, norm2_w,
  * fc1_w[mlp][h], fc1_b, fc2_w[h][mlp], fc2_b, ls2}, pool.{norm_q_w, norm_q_b, norm_k_w, norm_k_b, norm_v_w, norm_v_b, q_w[h][h], q_b,
  * k_w, k_b, v_w, v_b, proj_w[clip_dim][h], proj_b}, vproj_w[embed_dim][clip_dim], vproj_b.  GEMM weights are stored as fp16; norms,
- * biases, LayerScale gammas, cls and pos stay fp32. */
+ * biases, LayerScale gammas, cls and pos stay fp32.  Lifecycle: see cb_vit_set_tensor. */
 int cb_iv2_set_tensor(cb_iv2* iv2, const char* name, const float* data, size_t count);
 /* Checks that every tensor arrived and sizes the workspace for batches of up to max_clips clips. */
 int cb_iv2_finalize(cb_iv2* iv2, int max_clips);
@@ -360,7 +363,8 @@ int cb_iv2_text_create(cb_ctx* ctx, const cb_iv2_text_cfg* cfg, cb_iv2_text** ou
 void cb_iv2_text_destroy(cb_iv2_text* text);
 /* Upload one named tensor (host fp32, row-major, `count` elements).  Names: tok_emb[vocab][h], pos_emb[max_pos][h], type_emb[h] (token
  * type 0), emb_ln_w, emb_ln_b, L<i>.{qkv_w[3h][h] (query | key | value), qkv_b[3h], proj_w[h][h], proj_b, ln1_w, ln1_b, fc1_w[mlp][h],
- * fc1_b, fc2_w[h][mlp], fc2_b, ln2_w, ln2_b}, tproj_w[embed_dim][h], tproj_b.  GEMM weights are stored as fp16, the rest stays fp32. */
+ * fc1_b, fc2_w[h][mlp], fc2_b, ln2_w, ln2_b}, tproj_w[embed_dim][h], tproj_b.  GEMM weights are stored as fp16, the rest stays fp32.
+ * Lifecycle: see cb_vit_set_tensor. */
 int cb_iv2_text_set_tensor(cb_iv2_text* text, const char* name, const float* data, size_t count);
 /* Checks that every tensor arrived and sizes the workspace for calls of up to max_texts texts (more are run in chunks) of up to max_len
  * tokens; max_len <= min(max_pos, 352), else CB_ERR_UNSUPPORTED. */
