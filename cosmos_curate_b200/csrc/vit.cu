@@ -177,17 +177,30 @@ static int forward_chunk(cb_vit* v, const void* patches, int n, float* emb, floa
   else
     rc = cb::assemble_tokens(ctx, v->patch_out, nullptr, w.f(POS), nullptr, nullptr, v->h, n, T, g2, d, c.ln_eps, s);
   if (rc) return rc;
+  // CLIP reads only the [CLS] row (token 0) of the last layer's output.  Every op after that layer's attention is row-local, so
+  // from there on it runs on the n [CLS] rows alone: the residual gathered into [n][d] fp32 (patch-embed output is dead by now) and
+  // the attention rows into [n][d] fp16 (qkv is dead once attention has read it).
+  float* h = v->h;
+  __half* attn = v->attn;
   for (int i = 0; i < c.layers; ++i) {
     if ((rc = cb::layernorm_f16(ctx, v->h, w.f(i, LN1_W), w.f(i, LN1_B), v->xn, rows, d, c.ln_eps, s))) return rc;
     if ((rc = cb::gemm_f16(ctx, v->xn, w.h(i, QKV_W), w.f(i, QKV_B), nullptr, nullptr, v->qkv, rows, 3 * d, d, CB_EPI_NONE, s))) return rc;
     if ((rc = cb::attention_f16(ctx, v->qkv, v->attn, n, T, c.heads, hd, s))) return rc;
-    if ((rc = cb::gemm_f16(ctx, v->attn, w.h(i, OUT_W), w.f(i, OUT_B), v->h, v->h, nullptr, rows, d, d, CB_EPI_NONE, s))) return rc;
-    if ((rc = cb::layernorm_f16(ctx, v->h, w.f(i, LN2_W), w.f(i, LN2_B), v->xn, rows, d, c.ln_eps, s))) return rc;
-    if ((rc = cb::gemm_f16(ctx, v->xn, w.h(i, FC1_W), w.f(i, FC1_B), nullptr, nullptr, v->mlp, rows, c.mlp, d, act, s))) return rc;
-    if ((rc = cb::gemm_f16(ctx, v->mlp, w.h(i, FC2_W), w.f(i, FC2_B), v->h, v->h, nullptr, rows, d, c.mlp, CB_EPI_NONE, s))) return rc;
+    int m = rows;
+    if (c.arch == CB_ARCH_CLIP && i == c.layers - 1) {
+      h = v->patch_out, attn = v->qkv, m = n;
+      CB_CUDA(ctx, cudaMemcpy2DAsync(h, (size_t)d * sizeof(float), v->h, (size_t)T * d * sizeof(float), (size_t)d * sizeof(float), n,
+                                     cudaMemcpyDeviceToDevice, s));
+      CB_CUDA(ctx, cudaMemcpy2DAsync(attn, (size_t)d * sizeof(__half), v->attn, (size_t)T * d * sizeof(__half), (size_t)d * sizeof(__half), n,
+                                     cudaMemcpyDeviceToDevice, s));
+    }
+    if ((rc = cb::gemm_f16(ctx, attn, w.h(i, OUT_W), w.f(i, OUT_B), h, h, nullptr, m, d, d, CB_EPI_NONE, s))) return rc;
+    if ((rc = cb::layernorm_f16(ctx, h, w.f(i, LN2_W), w.f(i, LN2_B), v->xn, m, d, c.ln_eps, s))) return rc;
+    if ((rc = cb::gemm_f16(ctx, v->xn, w.h(i, FC1_W), w.f(i, FC1_B), nullptr, nullptr, v->mlp, m, c.mlp, d, act, s))) return rc;
+    if ((rc = cb::gemm_f16(ctx, v->mlp, w.h(i, FC2_W), w.f(i, FC2_B), h, h, nullptr, m, d, c.mlp, CB_EPI_NONE, s))) return rc;
   }
   if (c.arch == CB_ARCH_CLIP)
-    return cb::clip_tail(ctx, v->h, (size_t)T * d, w.f(POST_LN_W), w.f(POST_LN_B), c.proj_dim > 0 ? w.f(PROJ_W) : nullptr, d, c.proj_dim, c.ln_eps,
+    return cb::clip_tail(ctx, h, (size_t)d, w.f(POST_LN_W), w.f(POST_LN_B), c.proj_dim > 0 ? w.f(PROJ_W) : nullptr, d, c.proj_dim, c.ln_eps,
                          score ? v->aes_w : nullptr, v->aes_b, emb, feat, score, n, s);
   // SigLIP: post_layernorm on every token, then the MAP head (one learned query attends over the tokens, + MLP block)
   const __half* kv_w = (const __half*)w.h(MAP_IN_W) + (size_t)d * d;  // rows d..3d of in_proj_weight: K | V projections
