@@ -135,6 +135,13 @@ SIGNATURES = {
     "cb_attention_masked_f16": (_i, [_vp, _vp, _vp, _i, _i, _i, _i, _vp, _vp]),
     "cb_layernorm_post_f16": (_i, [_vp, _vp, _vp, _vp, _vp, _i, _i, _f, _vp]),
     "cb_text_embed": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _vp]),
+    "cb_assemble_tokens": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _f, _vp]),
+    "cb_clip_tail": (_i, [_vp, _vp, C.c_size_t, _vp, _vp, _vp, _i, _i, _f, _vp, _f, _vp, _vp, _vp, _i, _vp]),
+    "cb_map_pool": (_i, [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _vp]),
+    "cb_l2norm_score": (_i, [_vp, _vp, _i, _vp, _f, _vp, _vp, _vp, _i, _vp]),
+    "cb_token_mean": (_i, [_vp, _vp, _vp, _i, _i, _i, _vp]),
+    "cb_clip_pool": (_i, [_vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _vp]),
+    "cb_tube_patches": (_i, [_vp, _vp, _vp, _i, _i, _i, _i, _vp]),
     "cb_iv2_text_create": (_i, [_vp, C.POINTER(Iv2TextCfg), C.POINTER(_vp)]),
     "cb_iv2_text_destroy": (None, [_vp]),
     "cb_iv2_text_set_tensor": (_i, [_vp, C.c_char_p, _pf, C.c_size_t]),

@@ -710,6 +710,8 @@ __global__ void __launch_bounds__(256) clip_pool_kernel(const float* __restrict_
 }
 
 // ------------------------------------------------------------------------------------------ host
+static bool aligned(const void* p, uintptr_t bytes) { return ((uintptr_t)p & (bytes - 1)) == 0; }  // NULL counts as aligned
+
 int affine_score(cb_ctx* ctx, const float* emb, const float* w, float b, float* out, int n, int d, cudaStream_t stream) {
   if (!emb || !w || !out) return fail(ctx, CB_ERR_ARG, "affine_score: null operand");
   if (n <= 0) return CB_OK;
@@ -721,8 +723,11 @@ int affine_score(cb_ctx* ctx, const float* emb, const float* w, float b, float* 
 
 int layernorm_f16(cb_ctx* ctx, const float* x, const float* gamma, const float* beta, void* y, int rows, int d, float eps, cudaStream_t stream) {
   if (!x || !gamma || !beta || !y) return fail(ctx, CB_ERR_ARG, "layernorm: null operand");
-  if (rows <= 0) return CB_OK;
-  if (d % 128 || d > 128 * kLnMaxChunks) return fail(ctx, CB_ERR_UNSUPPORTED, "layernorm: d=%d must be a multiple of 128 and <= %d", d, 128 * kLnMaxChunks);
+  if (rows < 0) return fail(ctx, CB_ERR_ARG, "layernorm: rows=%d", rows);
+  if (d <= 0 || d % 128 || d > 128 * kLnMaxChunks) return fail(ctx, CB_ERR_UNSUPPORTED, "layernorm: d=%d must be a multiple of 128 and <= %d", d, 128 * kLnMaxChunks);
+  if (!aligned(x, 16) || !aligned(gamma, 16) || !aligned(beta, 16) || !aligned(y, 8))
+    return fail(ctx, CB_ERR_ARG, "layernorm: x, gamma, beta must be 16-byte and y 8-byte aligned");
+  if (rows == 0) return CB_OK;
   mark_launch(ctx, CB_PROF_LAYERNORM, stream);
   const unsigned grid = (unsigned)((rows + 7) / 8);
   switch (d >> 7) {  // ViT-B 768, ViT-L 1024, SoViT-400m 1152
@@ -739,6 +744,8 @@ int layernorm_post_f16(cb_ctx* ctx, float* h, const float* gamma, const float* b
   if (!h || !gamma || !beta || !y) return fail(ctx, CB_ERR_ARG, "layernorm_post: null operand");
   if (rows < 0) return fail(ctx, CB_ERR_ARG, "layernorm_post: rows=%d", rows);
   if (d <= 0 || d % 128 || d > 128 * kLnMaxChunks) return fail(ctx, CB_ERR_UNSUPPORTED, "layernorm_post: d=%d must be a multiple of 128 and <= %d", d, 128 * kLnMaxChunks);
+  if (!aligned(h, 16) || !aligned(gamma, 16) || !aligned(beta, 16) || !aligned(y, 8))
+    return fail(ctx, CB_ERR_ARG, "layernorm_post: h, gamma, beta must be 16-byte and y 8-byte aligned");
   if (rows == 0) return CB_OK;
   mark_launch(ctx, CB_PROF_LAYERNORM, stream);
   const unsigned grid = (unsigned)((rows + 7) / 8);
@@ -752,7 +759,15 @@ int layernorm_post_f16(cb_ctx* ctx, float* h, const float* gamma, const float* b
 
 int assemble_tokens(cb_ctx* ctx, const float* patch, const float* cls, const float* pos, const float* gamma, const float* beta, float* h, int n,
                     int tokens, int grid2, int d, float eps, cudaStream_t stream) {
-  if (d % 128 || d > 128 * kLnMaxChunks) return fail(ctx, CB_ERR_UNSUPPORTED, "assemble: d=%d unsupported", d);
+  if (!patch || !pos || !h || !gamma != !beta) return fail(ctx, CB_ERR_ARG, "assemble: null operand (gamma and beta go together)");
+  if (n < 0 || grid2 <= 0 || (tokens != grid2 && tokens != grid2 + 1))
+    return fail(ctx, CB_ERR_ARG, "assemble: n=%d tokens=%d grid2=%d (tokens is grid2, or grid2 + 1 with [CLS])", n, tokens, grid2);
+  if (tokens != grid2 && !cls) return fail(ctx, CB_ERR_ARG, "assemble: tokens=%d = grid2 + 1 needs the [CLS] row", tokens);
+  if ((size_t)n * tokens > (size_t)INT32_MAX) return fail(ctx, CB_ERR_UNSUPPORTED, "assemble: n * tokens = %zu rows", (size_t)n * tokens);
+  if (d <= 0 || d % 128 || d > 128 * kLnMaxChunks) return fail(ctx, CB_ERR_UNSUPPORTED, "assemble: d=%d must be a multiple of 128 and <= %d", d, 128 * kLnMaxChunks);
+  if (!aligned(patch, 16) || !aligned(cls, 16) || !aligned(pos, 16) || !aligned(gamma, 16) || !aligned(beta, 16) || !aligned(h, 16))
+    return fail(ctx, CB_ERR_ARG, "assemble: every operand must be 16-byte aligned");
+  if (n == 0) return CB_OK;
   const int rows = n * tokens;
   mark_launch(ctx, CB_PROF_OTHER, stream);
   assemble_kernel<<<(rows + 7) / 8, 256, 0, stream>>>(patch, cls, pos, gamma, beta, h, n, tokens, grid2, d, eps);
@@ -809,19 +824,42 @@ int attention_masked_f16(cb_ctx* ctx, const void* qkv, void* out, int n, int tok
   return CB_OK;
 }
 
+// The pools' shared memory: [tokens] probabilities, then max(1, 256 / head_dim) slices of head_dim partial sums, beside the static red[32].
+static int pool_smem(cb_ctx* ctx, const char* what, const void* kernel, int tokens, int head_dim, size_t* smem) {
+  if (head_dim <= 0 || head_dim % 2 || head_dim > 256)
+    return fail(ctx, CB_ERR_UNSUPPORTED, "%s: head_dim=%d must be even and <= 256 (one thread per output dimension)", what, head_dim);
+  const int slices = std::max(1, 256 / head_dim);
+  *smem = (size_t)(tokens + slices * head_dim) * sizeof(float);
+  int optin = 0;
+  CB_CUDA(ctx, cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, ctx->device));
+  if (*smem + 32 * sizeof(float) > (size_t)optin)
+    return fail(ctx, CB_ERR_UNSUPPORTED, "%s: tokens=%d needs %zu bytes of shared memory, the device grants %d", what, tokens, *smem, optin);
+  if (*smem > 48 * 1024) CB_CUDA(ctx, cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)*smem));
+  return CB_OK;
+}
+
 int map_pool(cb_ctx* ctx, const void* kv, const float* q, void* out, int n, int tokens, int heads, int head_dim, cudaStream_t stream) {
-  const int threads = 256;
-  const int slices = threads / head_dim > 0 ? threads / head_dim : 1;
-  const size_t smem = (size_t)(tokens + slices * head_dim) * sizeof(float);
-  if (smem > 48 * 1024) CB_CUDA(ctx, cudaFuncSetAttribute(map_pool_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  if (!kv || !q || !out) return fail(ctx, CB_ERR_ARG, "map_pool: null operand");
+  if (n < 0 || tokens <= 0 || heads <= 0) return fail(ctx, CB_ERR_ARG, "map_pool: n=%d tokens=%d heads=%d", n, tokens, heads);
+  if (!aligned(kv, 4) || !aligned(q, 4) || !aligned(out, 2)) return fail(ctx, CB_ERR_ARG, "map_pool: kv and q must be 4-byte, out 2-byte aligned");
+  size_t smem = 0;
+  if (const int rc = pool_smem(ctx, "map_pool", (const void*)map_pool_kernel, tokens, head_dim, &smem)) return rc;
+  if (n == 0) return CB_OK;
   mark_launch(ctx, CB_PROF_OTHER, stream);
-  map_pool_kernel<<<n * heads, threads, smem, stream>>>((const __half*)kv, q, (__half*)out, tokens, heads, head_dim);
+  map_pool_kernel<<<n * heads, 256, smem, stream>>>((const __half*)kv, q, (__half*)out, tokens, heads, head_dim);
   CB_CUDA(ctx, cudaGetLastError());
   return CB_OK;
 }
 
 int l2norm_score(cb_ctx* ctx, const float* feat, int d, const float* aes_w, float aes_b, float* emb, float* feat_out, float* score, int n,
                  cudaStream_t stream) {
+  if (!feat || !emb) return fail(ctx, CB_ERR_ARG, "l2norm_score: null operand");
+  if (n < 0) return fail(ctx, CB_ERR_ARG, "l2norm_score: n=%d", n);
+  // one lane per element, scalar loads: any width works (the towers' embed_dim only has to be a multiple of 8)
+  if (d <= 0 || d > 128 * kLnMaxChunks) return fail(ctx, CB_ERR_UNSUPPORTED, "l2norm_score: d=%d must be in [1, %d]", d, 128 * kLnMaxChunks);
+  if (!aligned(feat, 4) || !aligned(emb, 4) || !aligned(aes_w, 4) || !aligned(feat_out, 4) || !aligned(score, 4))
+    return fail(ctx, CB_ERR_ARG, "l2norm_score: operands must be 4-byte aligned");
+  if (n == 0) return CB_OK;
   mark_launch(ctx, CB_PROF_OTHER, stream);
   l2norm_score_kernel<<<(n + 7) / 8, 256, 0, stream>>>(feat, d, aes_w, aes_b, emb, feat_out, score, n);
   CB_CUDA(ctx, cudaGetLastError());
@@ -830,8 +868,18 @@ int l2norm_score(cb_ctx* ctx, const float* feat, int d, const float* aes_w, floa
 
 int clip_tail(cb_ctx* ctx, const float* h, size_t img_stride, const float* gamma, const float* beta, const float* proj, int d, int proj_dim,
               float eps, const float* aes_w, float aes_b, float* emb_out, float* feat_out, float* score_out, int n, cudaStream_t stream) {
+  if (!h || !gamma || !beta || !emb_out) return fail(ctx, CB_ERR_ARG, "clip_tail: null operand");
+  if (n < 0 || (proj && proj_dim <= 0) || img_stride < (size_t)d)
+    return fail(ctx, CB_ERR_ARG, "clip_tail: n=%d proj_dim=%d img_stride=%zu (>= d)", n, proj_dim, img_stride);
+  if (d <= 0 || d % 128 || d > 128 * kLnMaxChunks) return fail(ctx, CB_ERR_UNSUPPORTED, "clip_tail: d=%d must be a multiple of 128 and <= %d", d, 128 * kLnMaxChunks);
+  if (!aligned(h, 4) || !aligned(gamma, 4) || !aligned(beta, 4) || !aligned(proj, 16) || !aligned(aes_w, 4) || !aligned(emb_out, 4) ||
+      !aligned(feat_out, 4) || !aligned(score_out, 4))
+    return fail(ctx, CB_ERR_ARG, "clip_tail: proj must be 16-byte aligned, every other operand 4-byte");
   const int out_dim = proj ? proj_dim : d;
   const size_t smem = (size_t)(d + out_dim) * sizeof(float);
+  if (smem + 32 * sizeof(float) > 48 * 1024)  // pooled row + features in the default dynamic shared memory, beside red[32]
+    return fail(ctx, CB_ERR_UNSUPPORTED, "clip_tail: d + out_dim = %d floats exceed 48 KB of shared memory", d + out_dim);
+  if (n == 0) return CB_OK;
   mark_launch(ctx, CB_PROF_OTHER, stream);
   clip_tail_kernel<<<n, 256, smem, stream>>>(h, img_stride, gamma, beta, proj, d, proj_dim, eps, aes_w, aes_b, emb_out, feat_out, score_out);
   CB_CUDA(ctx, cudaGetLastError());
@@ -870,6 +918,10 @@ int qk_rmsnorm_f16(cb_ctx* ctx, void* qkv, const float* wq, const float* wk, int
 }
 
 int tube_patches(cb_ctx* ctx, const float* tubes, void* out, int frames, int image_size, int patch, int k_pad, cudaStream_t stream) {
+  if (!tubes || !out) return fail(ctx, CB_ERR_ARG, "tube_patches: null operand");
+  if (frames < 0 || patch <= 0 || image_size < patch || k_pad % 2 || k_pad < 3 * patch * patch)
+    return fail(ctx, CB_ERR_ARG, "tube_patches: frames=%d image_size=%d patch=%d k_pad=%d (even, >= 3 patch^2)", frames, image_size, patch, k_pad);
+  if (!aligned(tubes, 4) || !aligned(out, 4)) return fail(ctx, CB_ERR_ARG, "tube_patches: tubes and out must be 4-byte aligned");
   const int g = image_size / patch;
   const size_t total = (size_t)frames * g * g * (k_pad / 2);
   if (total == 0) return CB_OK;
@@ -881,6 +933,12 @@ int tube_patches(cb_ctx* ctx, const float* tubes, void* out, int frames, int ima
 }
 
 int token_mean(cb_ctx* ctx, const float* h, float* out, int n, int tokens, int d, cudaStream_t stream) {
+  if (!h || !out) return fail(ctx, CB_ERR_ARG, "token_mean: null operand");
+  if (n < 0 || tokens <= 0) return fail(ctx, CB_ERR_ARG, "token_mean: n=%d tokens=%d", n, tokens);
+  if (n > 65535) return fail(ctx, CB_ERR_UNSUPPORTED, "token_mean: n=%d exceeds the grid's y extent", n);
+  if (d <= 0 || d % 128 || d > 128 * kLnMaxChunks) return fail(ctx, CB_ERR_UNSUPPORTED, "token_mean: d=%d must be a multiple of 128 and <= %d", d, 128 * kLnMaxChunks);
+  if (!aligned(h, 4) || !aligned(out, 4)) return fail(ctx, CB_ERR_ARG, "token_mean: h and out must be 4-byte aligned");
+  if (n == 0) return CB_OK;
   mark_launch(ctx, CB_PROF_OTHER, stream);
   token_mean_kernel<<<dim3((d + 127) / 128, n), 128, 0, stream>>>(h, out, tokens, d);
   CB_CUDA(ctx, cudaGetLastError());
@@ -888,13 +946,16 @@ int token_mean(cb_ctx* ctx, const float* h, float* out, int n, int tokens, int d
 }
 
 int clip_pool(cb_ctx* ctx, const float* q, const void* k, const void* v, void* out, int n, int tokens, int heads, int head_dim, cudaStream_t stream) {
-  const int threads = 256;
-  const int slices = threads / head_dim > 0 ? threads / head_dim : 1;
-  const size_t smem = (size_t)(tokens + std::max(1, slices) * head_dim) * sizeof(float);
-  if (smem > 48 * 1024) CB_CUDA(ctx, cudaFuncSetAttribute(clip_pool_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  if (!q || !k || !v || !out) return fail(ctx, CB_ERR_ARG, "clip_pool: null operand");
+  if (n < 0 || tokens <= 0 || heads <= 0) return fail(ctx, CB_ERR_ARG, "clip_pool: n=%d tokens=%d heads=%d", n, tokens, heads);
+  if (!aligned(q, 4) || !aligned(k, 4) || !aligned(v, 2) || !aligned(out, 2))
+    return fail(ctx, CB_ERR_ARG, "clip_pool: q and k must be 4-byte, v and out 2-byte aligned");
+  size_t smem = 0;
+  if (const int rc = pool_smem(ctx, "clip_pool", (const void*)clip_pool_kernel, tokens, head_dim, &smem)) return rc;
+  if (n == 0) return CB_OK;
   mark_launch(ctx, CB_PROF_OTHER, stream);
-  clip_pool_kernel<<<n * heads, threads, smem, stream>>>(q, (const __half*)k, (const __half*)v, (__half*)out, tokens, heads, head_dim,
-                                                         1.0f / sqrtf((float)head_dim));
+  clip_pool_kernel<<<n * heads, 256, smem, stream>>>(q, (const __half*)k, (const __half*)v, (__half*)out, tokens, heads, head_dim,
+                                                     1.0f / sqrtf((float)head_dim));
   CB_CUDA(ctx, cudaGetLastError());
   return CB_OK;
 }
@@ -929,5 +990,36 @@ int cb_attention_masked_f16(cb_ctx* ctx, const void* qkv, void* out, int n, int 
 int cb_layernorm_post_f16(cb_ctx* ctx, float* h, const float* gamma, const float* beta, void* y, int rows, int d, float eps, void* stream) {
   if (!ctx) return CB_ERR_ARG;
   return cb::layernorm_post_f16(ctx, h, gamma, beta, y, rows, d, eps, (cudaStream_t)stream);
+}
+int cb_assemble_tokens(cb_ctx* ctx, const float* patch, const float* cls, const float* pos, const float* gamma, const float* beta, float* h, int n,
+                       int tokens, int grid2, int d, float eps, void* stream) {
+  if (!ctx) return CB_ERR_ARG;
+  return cb::assemble_tokens(ctx, patch, cls, pos, gamma, beta, h, n, tokens, grid2, d, eps, (cudaStream_t)stream);
+}
+int cb_clip_tail(cb_ctx* ctx, const float* h, size_t img_stride, const float* gamma, const float* beta, const float* proj, int d, int proj_dim,
+                 float eps, const float* aes_w, float aes_b, float* emb_out, float* feat_out, float* score_out, int n, void* stream) {
+  if (!ctx) return CB_ERR_ARG;
+  return cb::clip_tail(ctx, h, img_stride, gamma, beta, proj, d, proj_dim, eps, aes_w, aes_b, emb_out, feat_out, score_out, n, (cudaStream_t)stream);
+}
+int cb_map_pool(cb_ctx* ctx, const void* kv, const float* q, void* out, int n, int tokens, int heads, int head_dim, void* stream) {
+  if (!ctx) return CB_ERR_ARG;
+  return cb::map_pool(ctx, kv, q, out, n, tokens, heads, head_dim, (cudaStream_t)stream);
+}
+int cb_l2norm_score(cb_ctx* ctx, const float* feat, int d, const float* aes_w, float aes_b, float* emb_out, float* feat_out, float* score_out, int n,
+                    void* stream) {
+  if (!ctx) return CB_ERR_ARG;
+  return cb::l2norm_score(ctx, feat, d, aes_w, aes_b, emb_out, feat_out, score_out, n, (cudaStream_t)stream);
+}
+int cb_token_mean(cb_ctx* ctx, const float* h, float* out, int n, int tokens, int d, void* stream) {
+  if (!ctx) return CB_ERR_ARG;
+  return cb::token_mean(ctx, h, out, n, tokens, d, (cudaStream_t)stream);
+}
+int cb_clip_pool(cb_ctx* ctx, const float* q, const void* k, const void* v, void* out, int n, int tokens, int heads, int head_dim, void* stream) {
+  if (!ctx) return CB_ERR_ARG;
+  return cb::clip_pool(ctx, q, k, v, out, n, tokens, heads, head_dim, (cudaStream_t)stream);
+}
+int cb_tube_patches(cb_ctx* ctx, const float* tubes, void* out, int frames, int image_size, int patch, int k_pad, void* stream) {
+  if (!ctx) return CB_ERR_ARG;
+  return cb::tube_patches(ctx, tubes, out, frames, image_size, patch, k_pad, (cudaStream_t)stream);
 }
 }

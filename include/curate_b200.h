@@ -324,6 +324,34 @@ int cb_layernorm_post_f16(cb_ctx* ctx, float* h, const float* gamma, const float
  * ids device int32 [n][L] (not range-checked here), word [vocab][d], pos [>= L][d], type [d].  d % 4 == 0. */
 int cb_text_embed(cb_ctx* ctx, const int32_t* ids, const float* word, const float* pos, const float* type, float* h, int n, int L, int d,
                   void* stream);
+/* The towers' row kernels, each as the tower launches it.  Every call checks its arguments before it launches: a null operand, n < 0 or a
+ * misaligned pointer is CB_ERR_ARG; a width or shared-memory request the kernel cannot serve is CB_ERR_UNSUPPORTED; n == 0 is a no-op.
+ * d % 128 == 0 and d <= 1536 wherever a row is a d-wide vector of float4s.
+ * Tokens of the residual stream h fp32 [n][tokens][d] (tokens = grid2, or grid2 + 1 with cls fp32 [d] as token 0): h[i][t] =
+ * patch[i][t'] + pos[t], then LayerNorm(.) * gamma + beta when gamma and beta are given (CLIP's pre_layrnorm; SigLIP and InternVideo2
+ * pass neither).  patch fp32 [n][grid2][d], pos [tokens][d]; every pointer 16-byte aligned. */
+int cb_assemble_tokens(cb_ctx* ctx, const float* patch, const float* cls, const float* pos, const float* gamma, const float* beta, float* h, int n,
+                       int tokens, int grid2, int d, float eps, void* stream);
+/* CLIP's pooled head on rows h + i * img_stride (img_stride >= d floats): post_layernorm, then proj fp32 [proj_dim][d] (16-byte aligned;
+ * NULL: out_dim = d, no projection), emb_out [n][out_dim] = feat / |feat|, feat_out (nullable) = feat, score_out (nullable, with aes_w
+ * [out_dim]) = aes_w . emb + aes_b.  (d + out_dim) * 4 bytes must fit 48 KB of shared memory. */
+int cb_clip_tail(cb_ctx* ctx, const float* h, size_t img_stride, const float* gamma, const float* beta, const float* proj, int d, int proj_dim,
+                 float eps, const float* aes_w, float aes_b, float* emb_out, float* feat_out, float* score_out, int n, void* stream);
+/* SigLIP's MAP head attention: out fp16 [n][heads * head_dim] = softmax_t(q_h . k_t) v_t per (image, head), kv fp16 [n][tokens][2 *
+ * hidden] (k | v, 4-byte aligned), q fp32 [hidden] already scaled by head_dim^-1/2.  head_dim even and <= 256. */
+int cb_map_pool(cb_ctx* ctx, const void* kv, const float* q, void* out, int n, int tokens, int heads, int head_dim, void* stream);
+/* emb_out [n][d] = feat / |feat| per row, feat_out (nullable) = feat, score_out (nullable, with aes_w [d]) = aes_w . emb + aes_b.
+ * 1 <= d <= 1536, any width. */
+int cb_l2norm_score(cb_ctx* ctx, const float* feat, int d, const float* aes_w, float aes_b, float* emb_out, float* feat_out, float* score_out, int n,
+                    void* stream);
+/* out fp32 [n][d] = the mean over tokens of h fp32 [n][tokens][d], tokens summed in order (tokens >= 1, n <= 65535). */
+int cb_token_mean(cb_ctx* ctx, const float* h, float* out, int n, int tokens, int d, void* stream);
+/* InternVideo2's attention pooling, one query per clip: out fp16 [n][hidden] = softmax_t(head_dim^-1/2 q_h . k_t) v_t per (clip, head),
+ * q fp32 [n][hidden], k (4-byte aligned) and v fp16 [n][tokens][hidden].  head_dim even and <= 256. */
+int cb_clip_pool(cb_ctx* ctx, const float* q, const void* k, const void* v, void* out, int n, int tokens, int heads, int head_dim, void* stream);
+/* InternVideo2's patch rows: fp32 tubes [frames][3][S][S] -> fp16 [frames][(S / P)^2][k_pad], k = (c, y, x) of the P x P patch, zeros
+ * from 3 P^2 to k_pad.  k_pad even and >= 3 P^2, S >= P. */
+int cb_tube_patches(cb_ctx* ctx, const float* tubes, void* out, int frames, int image_size, int patch, int k_pad, void* stream);
 
 /* ---- InternVideo2 video tower (clip embeddings) ------------------------------------------------------ */
 /* The vision half of InternVideo2_Stage2.get_vid_feat (models/internvideo2_mm.py:203-217): PretrainInternVideo2.forward
