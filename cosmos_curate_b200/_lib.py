@@ -93,6 +93,7 @@ SIGNATURES = {
     "cb_preprocess_bilinear_u8": (_i, [_vp, C.POINTER(SurfacePool), _pi32, _i, _i, _i, _vp, _vp]),
     "cb_resize_cubic_u8": (_i, [_vp, C.POINTER(SurfacePool), _pi32, _i, _i, _i, _i, _vp, _vp]),
     "cb_video_tube": (_i, [_vp, C.POINTER(SurfacePool), _pi32, _i, _i, _i, _pf, _pf, _vp, _vp, _vp]),
+    "cb_video_tube_patches": (_i, [_vp, C.POINTER(SurfacePool), _pi32, _i, _i, _i, _i, _pf, _pf, _vp, _vp]),
     "cb_nv12_to_rgb": (_i, [_vp, C.POINTER(SurfacePool), _pi32, _i, _vp, _vp]),
     "cb_vit_create": (_i, [_vp, C.POINTER(VitCfg), C.POINTER(_vp)]),
     "cb_vit_destroy": (None, [_vp]),
@@ -132,6 +133,7 @@ SIGNATURES = {
     "cb_iv2_set_tensor": (_i, [_vp, C.c_char_p, _pf, C.c_size_t]),
     "cb_iv2_finalize": (_i, [_vp, _i]),
     "cb_iv2_forward": (_i, [_vp, _vp, _i, _vp, _vp]),
+    "cb_iv2_embed_surfaces": (_i, [_vp, C.POINTER(SurfacePool), _pi32, _i, _pf, _pf, _vp, _vp]),
     "cb_attention_masked_f16": (_i, [_vp, _vp, _vp, _i, _i, _i, _i, _vp, _vp]),
     "cb_layernorm_post_f16": (_i, [_vp, _vp, _vp, _vp, _vp, _i, _i, _f, _vp]),
     "cb_text_embed": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _vp]),

@@ -90,6 +90,10 @@ int ensure_norm_lut(cb_ctx* ctx, const float mean[3], const float std_[3], cudaS
 int bilinear_from_surface(cb_ctx* ctx, const void* base, int pitch, int luma_rows, int w, int h, int out_w, int out_h, uint8_t* out, cudaStream_t stream);
 int run_clip_preprocess(cb_ctx* ctx, const cb_surface_pool* pool, const int32_t* slots, int n, int res, int out_mode, int layout_patch,
                         int k_pad, int dtype, const float mean[3], const float std_[3], void* out, cudaStream_t stream);
+// cb_video_tube's resize + normalise of n frames of `pool` to size x size, written as the video tower's fp16 patch rows
+// [n][(size / patch)^2][k_pad] (pad columns zeroed).  n == 0 is a no-op.
+int video_tube_patches(cb_ctx* ctx, const cb_surface_pool* pool, const int32_t* slots, int n, int size, int patch, int k_pad, const float mean[3],
+                       const float std_[3], void* out_f16, cudaStream_t stream);
 
 // Tower ops (gemm.cu, vit_kernels.cu, attention_*.cu): fp16 operands, fp32 accumulation, launched on `stream`.
 int gemm_f16(cb_ctx* ctx, const void* A, const void* W, const float* bias, const float* residual, float* out_f32, void* out_f16, int M,

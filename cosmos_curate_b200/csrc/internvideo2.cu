@@ -4,7 +4,7 @@
 // (:596-650), vision_proj, L2 norm.
 //
 // Per clip of T frames (tokens = T * 256 + 1, head_dim 88):
-//   tube -> patch rows (k = (c, y, x), padded) -> GEMM + bias -> [CLS] + pos_embed
+//   tube (cb_iv2_forward) or decoded surfaces (cb_iv2_embed_surfaces) -> patch rows (k = (c, y, x), padded) -> GEMM + bias -> [CLS] + pos_embed
 //   40 x { RMSNorm -> qkv GEMM -> q/k RMSNorm (all heads together) -> streamed attention -> proj GEMM + bias, * ls1, + residual
 //          RMSNorm -> fc1 GEMM + bias, erf GELU -> fc2 GEMM + bias, * ls2, + residual }
 //   pooling: q = Wq LN_q(mean of the tokens) + bq, k = Wk LN_k(x) + bk, v = Wv LN_v(x) + bv, one query per clip, proj -> 768
@@ -125,14 +125,14 @@ int cb_iv2_finalize(cb_iv2* v, int max_clips) {
   return CB_OK;
 }
 
-static int forward_chunk(cb_iv2* v, const float* tubes, int n, float* emb, cudaStream_t s) {
+// The tower from the n clips' patch rows in v->patches on.
+static int forward_patches_chunk(cb_iv2* v, int n, float* emb, cudaStream_t s) {
   cb_ctx* ctx = v->ctx;
   const cb_iv2_cfg& c = v->cfg;
   const cb::WeightStore& w = v->w;
   const int d = c.hidden, T = v->tokens, rows = n * T, hd = d / c.heads;
   int rc;
   // patch embed: Conv3d(k = (1, p, p), stride = kernel, bias) as a GEMM over the patch rows, then [CLS] + pos_embed (no norm)
-  if ((rc = cb::tube_patches(ctx, tubes, v->patches, n * c.frames, c.image_size, c.patch, v->k_pad, s))) return rc;
   if ((rc = cb::gemm_f16(ctx, v->patches, w.h(PATCH_W), w.f(PATCH_B), nullptr, v->patch_out, nullptr, n * v->grid2, d, v->k_pad, CB_EPI_NONE, s)))
     return rc;
   if ((rc = cb::assemble_tokens(ctx, v->patch_out, w.f(CLS), w.f(POS), nullptr, nullptr, v->h, n, T, v->grid2, d, c.ln_eps, s))) return rc;
@@ -166,6 +166,11 @@ static int forward_chunk(cb_iv2* v, const float* tubes, int n, float* emb, cudaS
   return cb::l2norm_score(ctx, v->feat, c.embed_dim, nullptr, 0.f, emb, nullptr, nullptr, n, s);
 }
 
+static int forward_chunk(cb_iv2* v, const float* tubes, int n, float* emb, cudaStream_t s) {
+  const int rc = cb::tube_patches(v->ctx, tubes, v->patches, n * v->cfg.frames, v->cfg.image_size, v->cfg.patch, v->k_pad, s);
+  return rc ? rc : forward_patches_chunk(v, n, emb, s);
+}
+
 int cb_iv2_forward(cb_iv2* v, const float* tubes, int n, float* emb_out, void* stream) {
   if (!v) return CB_ERR_ARG;
   cb_ctx* ctx = v->ctx;
@@ -174,6 +179,20 @@ int cb_iv2_forward(cb_iv2* v, const float* tubes, int n, float* emb_out, void* s
   const size_t per_clip = (size_t)v->cfg.frames * 3 * v->cfg.image_size * v->cfg.image_size;
   return cb::for_chunks(n, v->max_clips, [&](int i, int m) {
     return forward_chunk(v, tubes + (size_t)i * per_clip, m, emb_out + (size_t)i * v->cfg.embed_dim, (cudaStream_t)stream);
+  });
+}
+
+int cb_iv2_embed_surfaces(cb_iv2* v, const cb_surface_pool* pool, const int32_t* slots, int n_clips, const float mean[3], const float std_[3],
+                          float* emb_out, void* stream) {
+  if (!v) return CB_ERR_ARG;
+  cb_ctx* ctx = v->ctx;
+  if (!v->finalized) return cb::fail(ctx, CB_ERR_STATE, "iv2_embed_surfaces before iv2_finalize");
+  if (n_clips < 0 || (n_clips > 0 && (!pool || !slots || !mean || !std_ || !emb_out))) return cb::fail(ctx, CB_ERR_ARG, "iv2_embed_surfaces: null argument");
+  const cb_iv2_cfg& c = v->cfg;
+  return cb::for_chunks(n_clips, v->max_clips, [&](int i, int m) {
+    const int rc = cb::video_tube_patches(ctx, pool, slots + (size_t)i * c.frames, m * c.frames, c.image_size, c.patch, v->k_pad, mean, std_,
+                                          v->patches, (cudaStream_t)stream);
+    return rc ? rc : forward_patches_chunk(v, m, emb_out + (size_t)i * c.embed_dim, (cudaStream_t)stream);
   });
 }
 

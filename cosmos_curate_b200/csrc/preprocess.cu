@@ -14,6 +14,7 @@
 //  nv12_to_rgb_kernel     : full-resolution NV12 -> RGB24.
 //  resize_cubic_kernel    : cv2.resize(INTER_CUBIC) of a surface's RGB image.
 //  video_tube_kernel      : cv2.resize(INTER_LINEAR) + normalise -> the video towers' fp32 input.
+//  video_tube_patches_kernel : the same pixels -> the video tower's fp16 patch rows (one launch from surfaces to the patch GEMM).
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
 
@@ -469,6 +470,8 @@ __global__ void resize_cubic_kernel(const CubicArgs a) {
 // OpenCV's fixed-point arithmetic, bit for bit: int16 weights at 2^11 (each of the pair rounded on its own), horizontal pass
 // in int32, vertical pass (((b0 * (S0 >> 4)) >> 16) + ((b1 * (S1 >> 4)) >> 16) + 2) >> 2; an exact 2x2 decimation is what
 // cv2 reroutes to INTER_AREA ((a + b + c + d + 2) >> 2); equal sizes copy.  HBM-bound and sparse: 4 source pixels per output.
+// Two kernels write it: video_tube_kernel (fp32 CHW and/or u8 HWC) and video_tube_patches_kernel (the video tower's fp16 patch
+// rows); both compute every pixel with tube_pixel and normalise it with the LUT of tube_norm_lut.
 struct TubeArgs {
   Surface s;
   int n, out_w, out_h, mode;  // mode 0 linear, 1 area 2x2, 2 copy
@@ -477,21 +480,22 @@ struct TubeArgs {
   float mean[3], std_[3];
   float* out_f32;    // [n][3][out_h][out_w] or null
   uint8_t* out_u8;   // [n][out_h][out_w][3] or null
+  __half* out_patch; // video_tube_patches_kernel: [n][(out_w / patch)^2][k_pad]
+  int patch, k_pad;
 };
 
-__global__ void video_tube_kernel(const TubeArgs a) {
-  __shared__ float lut[3][256];
+// lut[c][v] = ((v / 255) - mean[c]) / std[c] in fp32, the value the tube holds for channel c at u8 level v.  Ends in __syncthreads().
+__device__ __forceinline__ void tube_norm_lut(const TubeArgs& a, float (*lut)[256]) {
   for (int t = threadIdx.x; t < 768; t += blockDim.x) {
     const int c = t >> 8, v = t & 255;
     lut[c][v] = __fdiv_rn(__fsub_rn(__fdiv_rn((float)v, 255.0f), a.mean[c]), a.std_[c]);
   }
   __syncthreads();
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  const int per = a.out_w * a.out_h;
-  if (i >= a.n * per) return;
-  const int f = i / per, p = i - f * per, yo = p / a.out_w, xo = p - yo * a.out_w;
+}
+
+// The resized u8 RGB of output pixel (xo, yo) of frame f.
+__device__ __forceinline__ void tube_pixel(const TubeArgs& a, int f, int yo, int xo, int v[3]) {
   const uint8_t* fr = a.s.frame(f);
-  int v[3];
   if (a.mode == 2) {
     a.s.rgb(fr, xo, yo, v[0], v[1], v[2]);
   } else if (a.mode == 1) {
@@ -519,6 +523,17 @@ __global__ void video_tube_kernel(const TubeArgs a) {
       v[c] = (((b0 * (s0 >> 4)) >> 16) + ((b1 * (s1 >> 4)) >> 16) + 2) >> 2;
     }
   }
+}
+
+__global__ void video_tube_kernel(const TubeArgs a) {
+  __shared__ float lut[3][256];
+  tube_norm_lut(a, lut);
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  const int per = a.out_w * a.out_h;
+  if (i >= a.n * per) return;
+  const int f = i / per, p = i - f * per, yo = p / a.out_w, xo = p - yo * a.out_w;
+  int v[3];
+  tube_pixel(a, f, yo, xo, v);
   if (a.out_u8) {
     uint8_t* o = a.out_u8 + (size_t)i * 3;
     o[0] = (uint8_t)v[0], o[1] = (uint8_t)v[1], o[2] = (uint8_t)v[2];
@@ -528,6 +543,31 @@ __global__ void video_tube_kernel(const TubeArgs a) {
 #pragma unroll
     for (int c = 0; c < 3; ++c) o[(size_t)c * per] = lut[c][v[c] & 255];
   }
+}
+
+// The same tube straight into the video tower's patch rows: fp16 [n][G^2][k_pad] with G = out_w / patch and k = (c, y, x) of the
+// patch, zeros from 3 patch^2 to k_pad - each value __float2half_rn of what video_tube_kernel writes to out_f32, so this equals
+// tube_patches_kernel applied to that tube.  One thread per pixel of a patch (writing its three channels) or per pad column.
+__global__ void __launch_bounds__(256) video_tube_patches_kernel(const TubeArgs a) {
+  __shared__ float lut[3][256];
+  tube_norm_lut(a, lut);
+  const int P = a.patch, G = a.out_w / P, pp = P * P, kp = 3 * pp;
+  const int per_row = pp + (a.k_pad - kp);  // work items of one patch row: its pixels, then its pad columns
+  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= (long long)a.n * G * G * per_row) return;
+  const long long row = i / per_row;  // frame * G^2 + patch
+  const int e = (int)(i - row * per_row);
+  __half* o = a.out_patch + row * a.k_pad;
+  if (e >= pp) {
+    o[kp + (e - pp)] = __float2half_rn(0.f);
+    return;
+  }
+  const int f = (int)(row / (G * G)), patch = (int)(row - (long long)f * G * G);
+  const int py = patch / G, px = patch - py * G, y = e / P, x = e - y * P;
+  int v[3];
+  tube_pixel(a, f, py * P + y, px * P + x, v);
+#pragma unroll
+  for (int c = 0; c < 3; ++c) o[c * pp + e] = __float2half_rn(lut[c][v[c] & 255]);
 }
 
 
@@ -898,31 +938,60 @@ static int run_resize_cubic(cb_ctx* ctx, const cb_surface_pool* pool, const int3
   return CB_OK;
 }
 
+// The tube kernels' prologue: checks the request, describes the pool in `a`, picks the resize mode and its tap tables and uploads the
+// slots.  Returns 1 when there is nothing to launch (n == 0).
+static int open_tube(cb_ctx* ctx, const cb_surface_pool* pool, const int32_t* slots, int n, int out_w, int out_h, bool normalise,
+                     const float mean[3], const float std_[3], const void* out, TubeArgs* a, cudaStream_t stream) {
+  int rc = open_pool(ctx, pool, slots, n, out, &a->s, stream);
+  if (rc) return rc;
+  if (out_w <= 0 || out_h <= 0 || out_w > 8192 || out_h > 8192) return fail(ctx, CB_ERR_ARG, "bad output size %dx%d", out_w, out_h);
+  if (normalise && (!mean || !std_)) return fail(ctx, CB_ERR_ARG, "null mean/std");
+  if (is_nv12(pool->format) && ((pool->width | pool->height) & 1)) return fail(ctx, CB_ERR_UNSUPPORTED, "NV12 needs even dimensions");
+  if ((long long)n * out_w * out_h > 0x7fffffffLL) return fail(ctx, CB_ERR_ARG, "too many output pixels for one call");
+  a->n = n, a->out_w = out_w, a->out_h = out_h;
+  for (int c = 0; c < 3; ++c) a->mean[c] = mean ? mean[c] : 0.f, a->std_[c] = std_ ? std_[c] : 1.f;
+  if (a->s.w == out_w && a->s.h == out_h) {
+    a->mode = 2;
+  } else if (a->s.w == 2 * out_w && a->s.h == 2 * out_h) {
+    a->mode = 1;
+  } else {
+    a->mode = 0;
+    const ResizeTaps* tx = get_resize_taps(ctx, a->s.w, out_w, kTapsLinearZeroBorder);
+    const ResizeTaps* ty = get_resize_taps(ctx, a->s.h, out_h, kTapsLinearClamp);
+    if (!tx || !ty) return fail(ctx, CB_ERR_CUDA, "linear tap table allocation failed");
+    a->x0 = tx->d_first, a->ax = tx->d_wq, a->y0 = ty->d_first, a->by = ty->d_wq;
+  }
+  return CB_OK;
+}
+
 static int run_video_tube(cb_ctx* ctx, const cb_surface_pool* pool, const int32_t* slots, int n, int out_w, int out_h, const float mean[3],
                           const float std_[3], float* out_f32, uint8_t* out_u8, cudaStream_t stream) {
   TubeArgs a{};
-  int rc = open_pool(ctx, pool, slots, n, out_f32 ? (const void*)out_f32 : out_u8, &a.s, stream);
+  int rc = open_tube(ctx, pool, slots, n, out_w, out_h, out_f32 != nullptr, mean, std_, out_f32 ? (const void*)out_f32 : out_u8, &a, stream);
   if (rc) return rc > 0 ? CB_OK : rc;
-  if (out_w <= 0 || out_h <= 0 || out_w > 8192 || out_h > 8192) return fail(ctx, CB_ERR_ARG, "bad output size %dx%d", out_w, out_h);
-  if (out_f32 && (!mean || !std_)) return fail(ctx, CB_ERR_ARG, "null mean/std");
-  if (is_nv12(pool->format) && ((pool->width | pool->height) & 1)) return fail(ctx, CB_ERR_UNSUPPORTED, "NV12 needs even dimensions");
-  if ((long long)n * out_w * out_h > 0x7fffffffLL) return fail(ctx, CB_ERR_ARG, "too many output pixels for one call");
-  a.n = n, a.out_w = out_w, a.out_h = out_h, a.out_f32 = out_f32, a.out_u8 = out_u8;
-  for (int c = 0; c < 3; ++c) a.mean[c] = mean ? mean[c] : 0.f, a.std_[c] = std_ ? std_[c] : 1.f;
-  if (a.s.w == out_w && a.s.h == out_h) {
-    a.mode = 2;
-  } else if (a.s.w == 2 * out_w && a.s.h == 2 * out_h) {
-    a.mode = 1;
-  } else {
-    a.mode = 0;
-    const ResizeTaps* tx = get_resize_taps(ctx, a.s.w, out_w, kTapsLinearZeroBorder);
-    const ResizeTaps* ty = get_resize_taps(ctx, a.s.h, out_h, kTapsLinearClamp);
-    if (!tx || !ty) return fail(ctx, CB_ERR_CUDA, "linear tap table allocation failed");
-    a.x0 = tx->d_first, a.ax = tx->d_wq, a.y0 = ty->d_first, a.by = ty->d_wq;
-  }
+  a.out_f32 = out_f32, a.out_u8 = out_u8;
   mark_launch(ctx, CB_PROF_PREPROCESS, stream);
   const long long total = (long long)n * out_w * out_h;
   video_tube_kernel<<<(unsigned)((total + 255) / 256), 256, 0, stream>>>(a);
+  CB_CUDA(ctx, cudaGetLastError());
+  return CB_OK;
+}
+
+int video_tube_patches(cb_ctx* ctx, const cb_surface_pool* pool, const int32_t* slots, int n, int size, int patch, int k_pad, const float mean[3],
+                       const float std_[3], void* out_f16, cudaStream_t stream) {
+  if (!ctx) return CB_ERR_ARG;
+  if (patch <= 0 || size < patch || k_pad % 2 || k_pad < 3 * patch * patch)
+    return fail(ctx, CB_ERR_ARG, "video_tube_patches: size=%d patch=%d k_pad=%d (even, >= 3 patch^2)", size, patch, k_pad);
+  if ((uintptr_t)out_f16 & 1) return fail(ctx, CB_ERR_ARG, "video_tube_patches: out must be 2-byte aligned");
+  TubeArgs a{};
+  int rc = open_tube(ctx, pool, slots, n, size, size, true, mean, std_, out_f16, &a, stream);
+  if (rc) return rc > 0 ? CB_OK : rc;
+  a.out_patch = (__half*)out_f16, a.patch = patch, a.k_pad = k_pad;
+  const int g = size / patch;
+  const long long total = (long long)n * g * g * (patch * patch + k_pad - 3 * patch * patch);
+  if ((total + 255) / 256 > 0x7fffffffLL) return fail(ctx, CB_ERR_ARG, "video_tube_patches: too many frames for one call");
+  mark_launch(ctx, CB_PROF_PREPROCESS, stream);
+  video_tube_patches_kernel<<<(unsigned)((total + 255) / 256), 256, 0, stream>>>(a);
   CB_CUDA(ctx, cudaGetLastError());
   return CB_OK;
 }
@@ -974,6 +1043,11 @@ int cb_video_tube(cb_ctx* ctx, const cb_surface_pool* pool, const int32_t* slots
                   const float std_[3], float* out_f32, uint8_t* out_u8, void* stream) {
   if (!ctx) return CB_ERR_ARG;
   return cb::run_video_tube(ctx, pool, slots, n, out_w, out_h, mean, std_, out_f32, out_u8, (cudaStream_t)stream);
+}
+
+int cb_video_tube_patches(cb_ctx* ctx, const cb_surface_pool* pool, const int32_t* slots, int n, int size, int patch, int k_pad, const float mean[3],
+                          const float std_[3], void* out_f16, void* stream) {
+  return cb::video_tube_patches(ctx, pool, slots, n, size, patch, k_pad, mean, std_, out_f16, (cudaStream_t)stream);
 }
 
 int cb_nv12_to_rgb(cb_ctx* ctx, const cb_surface_pool* pool, const int32_t* slots, int n, uint8_t* out, void* stream) {

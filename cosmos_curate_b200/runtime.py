@@ -405,6 +405,18 @@ class Iv2Tower(_Handle):
         check(self.lib.cb_iv2_forward(self.h, tubes.data_ptr(), tubes.shape[0], out.data_ptr(), _stream_ptr()), "cb_iv2_forward", self.ctx.h)
         return out
 
+    def embed_pool(self, pool: Pool, slots, mean=IMAGENET_MEAN, std=IMAGENET_STD) -> torch.Tensor:
+        """Decoded frames -> unit-norm float32 cuda [n_clips, embed_dim]: `slots` holds n_clips * frames surface indices of `pool`,
+        clip-major (repeats allowed).  Bitwise forward(video_tube(pool, S, S, slots).view(n_clips, frames, 3, S, S))."""
+        arr, ptr = self.ctx._slots(pool, slots)
+        if len(arr) % self.frames:
+            raise ValueError(f"{len(arr)} slots are not whole clips of {self.frames} frames")
+        n = len(arr) // self.frames
+        out = torch.empty((n, self.embed_dim), dtype=torch.float32, device=pool.buf.device)
+        check(self.lib.cb_iv2_embed_surfaces(self.h, C.byref(pool.desc), ptr, n, _f3(mean), _f3(std), out.data_ptr(), _stream_ptr()),
+              "cb_iv2_embed_surfaces", self.ctx.h)  # fmt: skip
+        return out
+
 
 class Iv2TextTower(_Handle):
     """cb_iv2_text_* wrapper: weights in (fp32 numpy, names of include/curate_b200.h cb_iv2_text_set_tensor), text embeddings out."""

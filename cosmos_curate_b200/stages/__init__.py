@@ -16,6 +16,7 @@ New fused stage (replaces ClipFrameExtractionStage -> AestheticFilterStage [-> c
     NvdecClipAestheticStage
     NvdecShotDetectionStage      (VideoFrameExtractionStage -> TransNetV2ClipExtractionStage, frames stay in HBM)
     ClipStreamCopyStage          (ClipTranscodingStage without the transcode: clip mp4s by stream copy, clip_extraction_stages.py:167-442)
+    NvdecInternVideo2EmbeddingStage  (InternVideo2FrameCreationStage(source="nvdec") -> InternVideo2EmbeddingStage, tubes stay in HBM)
 """
 
 from .aesthetic_filter import AestheticFilterStage  # noqa: F401
@@ -28,5 +29,6 @@ from .fused_clip import NvdecClipAestheticStage  # noqa: F401
 from .frame_extraction import ClipFrameExtractionStage, VideoFrameExtractionStage  # noqa: F401
 from .internvideo2_embedding import InternVideo2EmbeddingStage  # noqa: F401
 from .internvideo2_frames import InternVideo2FrameCreationStage  # noqa: F401
+from .internvideo2_fused import NvdecInternVideo2EmbeddingStage  # noqa: F401
 from .image_embedding import ImageCLIPEmbeddingStage  # noqa: F401
 from .transnetv2_extraction import NvdecShotDetectionStage, TransNetV2ClipExtractionStage  # noqa: F401

@@ -18,38 +18,47 @@ from ..interfaces import CuratorStage, CuratorStageResource, ModelInterface
 from ..models.internvideo2 import InternVideo2MultiModality
 
 
+class TextMatch:
+    """`texts_to_verify` of the InternVideo2 embedding stages: the constructor refuses an empty list and a model that cannot embed text,
+    embed() embeds the texts once (stage_setup), verify(clip) sets clip.intern_video_2_text_match on a clip that has an embedding."""
+
+    def __init__(self, model, texts_to_verify: list[str] | None) -> None:
+        if texts_to_verify is not None:
+            if not texts_to_verify:
+                msg = "texts_to_verify is empty: give at least one text, or None"
+                raise ValueError(msg)
+            if not (callable(getattr(model, "encode_texts", None)) and callable(getattr(model, "evaluate", None))):
+                msg = f"texts_to_verify needs a model that embeds text (encode_texts / evaluate); {type(model).__name__} does not"
+                raise ValueError(msg)
+        self._model = model
+        self._texts = list(texts_to_verify) if texts_to_verify is not None else None
+        self._text_embeddings = None
+
+    def embed(self):
+        if self._texts is not None and self._text_embeddings is None:
+            self._text_embeddings = list(self._model.encode_texts(self._texts))
+        return self._text_embeddings
+
+    def verify(self, clip) -> None:
+        if self._texts is not None and clip.intern_video_2_embedding is not None:
+            probs, idxs = self._model.evaluate(clip.intern_video_2_embedding, self.embed())
+            clip.intern_video_2_text_match = (self._texts[idxs[0]], probs[0])
+
+
 class InternVideo2EmbeddingStage(CuratorStage):
     """Stage for generating embeddings from InternVideo2 input frames."""
 
     def __init__(self, num_gpus_per_worker: float = 0.25, batch_size: int = 8, *, verbose: bool = False, log_stats: bool = False,
                  texts_to_verify: list[str] | None = None, model: InternVideo2MultiModality | None = None) -> None:  # fmt: skip
         self._model = model if model is not None else InternVideo2MultiModality()
-        if texts_to_verify is not None:
-            if not texts_to_verify:
-                msg = "texts_to_verify is empty: give at least one text, or None"
-                raise ValueError(msg)
-            if not (callable(getattr(self._model, "encode_texts", None)) and callable(getattr(self._model, "evaluate", None))):
-                msg = f"texts_to_verify needs a model that embeds text (encode_texts / evaluate); {type(self._model).__name__} does not"
-                raise ValueError(msg)
-        self._texts = list(texts_to_verify) if texts_to_verify is not None else None
-        self._text_embeddings = None
+        self._text_match = TextMatch(self._model, texts_to_verify)
         self._timer = StageTimer(self)
         self._num_gpus_per_worker, self._batch_size = num_gpus_per_worker, batch_size
         self._verbose, self._log_stats = verbose, log_stats
 
     def stage_setup(self) -> None:
         self._model.setup()
-        self._embed_texts()
-
-    def _embed_texts(self):
-        if self._texts is not None and self._text_embeddings is None:
-            self._text_embeddings = list(self._model.encode_texts(self._texts))
-        return self._text_embeddings
-
-    def _verify_with_texts(self, clip) -> None:
-        if self._texts is not None and clip.intern_video_2_embedding is not None:
-            probs, idxs = self._model.evaluate(clip.intern_video_2_embedding, self._embed_texts())
-            clip.intern_video_2_text_match = (self._texts[idxs[0]], probs[0])
+        self._text_match.embed()
 
     @property
     def model(self) -> ModelInterface:
@@ -80,7 +89,7 @@ class InternVideo2EmbeddingStage(CuratorStage):
                     for clip, e in zip(todo, embeddings):
                         clip.intern_video_2_embedding = e
                 for clip in clips:
-                    self._verify_with_texts(clip)
+                    self._text_match.verify(clip)
             finally:
                 for clip in clips:
                     clip.intern_video_2_frames.drop()

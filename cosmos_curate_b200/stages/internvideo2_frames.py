@@ -49,6 +49,81 @@ def sampled_ids_with_regen(ts: np.ndarray, target_fps: float, target_num_frames:
     return ids, used
 
 
+def plan_clip(clip, data, target_fps: float, fn: int, verbose: bool = False):
+    """The decode plan of one clip's tube: -> (surface size, distinct frame ids to decode, slot of every kept frame relative to the
+    clip's first slot), None when the clip is too short (tube = the reference's empty array), or raises for an unreadable container.
+    The sampled ids come from the MP4 index, with the re-extraction rule applied to the id lists (sampled_ids_with_regen)."""
+    idx = mp4_index(data)
+    ts = sampling.timestamps_from_index(idx["pts"], idx["timescale"])
+    ids, fps = sampled_ids_with_regen(ts, target_fps, fn)
+    if len(ids) < fn:
+        logger.error(f"Clip {clip.uuid} is too short to extract enough frames.")
+        logger.error(f"Frame count {len(ids)} is smaller than minimal requirement {fn}")
+        return None
+    if verbose and fps != target_fps:
+        logger.warning(f"Clip {clip.uuid} has <{fn} frames at target_fps={target_fps}; sampled at {fps}.")
+    keep = np.asarray(ids)[select_frame_ids(len(ids), fn)]
+    uniq, inverse = np.unique(keep, return_inverse=True)  # a frame kept twice (supersampled clip) is decoded once
+    return even_size(idx["width"], idx["height"]), uniq.astype(np.int32), inverse.astype(np.int32)
+
+
+def run_decode_groups(items, plan, pools: SurfacePools, decoders, compute, *, on_short, on_error, group: int, depth: int = 2,
+                      seek_keyframes: bool = False, retire=None) -> tuple[int, int]:  # fmt: skip
+    """Decode the kept frames of clips [(clip, mp4 bytes)] into surface pools, group by group, and hand each group to `compute`.
+
+    plan(clip, data) gives plan_clip's result: None sends the clip to on_short(clip), CurateB200Error / ValueError to on_error(clip, e).
+    The planned clips are grouped per surface size, `group` clips at a time.  Group k is decoded by decoders() (a DecoderPool) into
+    pool k % depth of its size's ring while the groups before it compute.  compute(k, pool, clips, slots) gets the clips whose decode
+    succeeded (the others go to on_error) and their kept frames' surface indices, concatenated clip-major.  When compute only queues
+    GPU work, retire(k) must return once group k's work no longer reads its pool: a pool is decoded into again only after that.
+    -> (frames decoded, groups)."""
+    by_size: dict[tuple, list] = {}
+    for clip, data in items:
+        try:
+            planned = plan(clip, data)
+        except (CurateB200Error, ValueError) as e:
+            on_error(clip, e)
+            continue
+        if planned is None:
+            on_short(clip)
+            continue
+        by_size.setdefault(planned[0], []).append((clip, data, planned[1], planned[2]))
+    groups = [(size, clips[i : i + group]) for size, clips in by_size.items() for i in range(0, len(clips), group)]
+    ring_pos: dict[tuple, int] = {}
+    pending: dict[int, tuple] = {}
+
+    def submit(k):
+        size, clips = groups[k]
+        r = ring_pos.get(size, 0)
+        ring_pos[size] = (r + 1) % depth
+        pool = pools.get(size, sum(len(ids) for _, _, ids, _ in clips), r)
+        pending[k] = pool, decoders().submit_group(pool, size, [(data, ids) for _, data, ids, _ in clips], seek_keyframes)
+
+    decoded = 0
+    for k in range(min(depth - 1, len(groups))):
+        submit(k)
+    for k, (_, clips) in enumerate(groups):
+        pool, jobs = pending.pop(k)
+        n, errs = collect_group(jobs)
+        decoded += n
+        ok, slots = [], []
+        for (clip, _, _, inverse), (first, _), err in zip(clips, jobs, errs):
+            if err is not None:
+                on_error(clip, err)
+                continue
+            ok.append(clip)
+            slots.append(first + inverse)
+        if retire is not None and k >= 1:
+            retire(k - 1)
+        if k + depth - 1 < len(groups):
+            submit(k + depth - 1)  # the next groups decode while this one computes
+        if ok:
+            compute(k, pool, ok, np.concatenate(slots).astype(np.int32))
+    if retire is not None and groups:
+        retire(len(groups) - 1)
+    return decoded, len(groups)
+
+
 class InternVideo2FrameCreationStage(CuratorStage):
     """Stage for creating InternVideo2 input frames from video clips."""
 
@@ -101,64 +176,21 @@ class InternVideo2FrameCreationStage(CuratorStage):
             self._decode_pool = DecoderPool(self._ctx, self._num_decoders)
         return self._decode_pool
 
-    def _plan(self, clip, data):
-        """-> (size, distinct frame ids to decode, slot of every kept frame relative to the clip's first slot), None when the
-        clip is too short (tube = the reference's empty array), or raises for an unreadable container."""
-        idx = mp4_index(data)
-        ts = sampling.timestamps_from_index(idx["pts"], idx["timescale"])
-        fn = self._model.get_target_num_frames()
-        ids, fps = sampled_ids_with_regen(ts, self._target_fps, fn)
-        if len(ids) < fn:
-            logger.error(f"Clip {clip.uuid} is too short to extract enough frames.")
-            logger.error(f"Frame count {len(ids)} is smaller than minimal requirement {fn}")
-            return None
-        if self._verbose and fps != self._target_fps:
-            logger.warning(f"Clip {clip.uuid} has <{fn} frames at target_fps={self._target_fps}; sampled at {fps}.")
-        keep = np.asarray(ids)[select_frame_ids(len(ids), fn)]
-        uniq, inverse = np.unique(keep, return_inverse=True)  # a frame kept twice (supersampled clip) is decoded once
-        return even_size(idx["width"], idx["height"]), uniq.astype(np.int32), inverse.astype(np.int32)
-
     def _tubes_from_streams(self, items) -> None:
         """items: [(clip, data)].  Decode groups of GROUP clips on the session pool (group k+1 decodes while group k is
         resized, normalised and copied out), one tube kernel launch per group."""
         fn = self._model.get_target_num_frames()
-        by_size: dict[tuple, list] = {}
-        for clip, data in items:
-            try:
-                plan = self._plan(clip, data)
-            except (CurateB200Error, ValueError) as e:
-                self._decode_failed(clip, e)
-                continue
-            if plan is None:
-                clip.intern_video_2_frames = np.empty(0, dtype=np.float32)
-                continue
-            by_size.setdefault(plan[0], []).append((clip, data, plan[1], plan[2]))
-        groups = [(size, clips[i : i + self.GROUP]) for size, clips in by_size.items() for i in range(0, len(clips), self.GROUP)]
-        ring_pos: dict[tuple, int] = {}
 
-        def submit(k):
-            size, clips = groups[k]
-            r = ring_pos.get(size, 0)
-            ring_pos[size] = r ^ 1
-            pool = self._pools.get(size, sum(len(ids) for _, _, ids, _ in clips), r)
-            return pool, self._decoders().submit_group(pool, size, [(data, ids) for _, data, ids, _ in clips])
+        def too_short(clip):
+            clip.intern_video_2_frames = np.empty(0, dtype=np.float32)
 
-        pending = submit(0) if groups else None
-        for k, (_, clips) in enumerate(groups):
-            pool, jobs = pending
-            _, errs = collect_group(jobs)
-            ok, slots = [], []
-            for (clip, _, _, inverse), (first, _), err in zip(clips, jobs, errs):
-                if err is not None:
-                    self._decode_failed(clip, err)
-                    continue
-                ok.append(clip)
-                slots.append(first + inverse)
-            pending = submit(k + 1) if k + 1 < len(groups) else None  # next group's decode overlaps this group's kernel + D2H
-            if ok:
-                tubes = self._model.formulate_pool(pool, np.concatenate(slots)).cpu().numpy()  # [len(ok) * fn, 3, s, s]
-                for i, clip in enumerate(ok):
-                    clip.intern_video_2_frames = tubes[i * fn : (i + 1) * fn][None].copy()
+        def compute(k, pool, ok, slots):
+            tubes = self._model.formulate_pool(pool, slots).cpu().numpy()  # [len(ok) * fn, 3, s, s]
+            for i, clip in enumerate(ok):
+                clip.intern_video_2_frames = tubes[i * fn : (i + 1) * fn][None].copy()
+
+        run_decode_groups(items, lambda clip, data: plan_clip(clip, data, self._target_fps, fn, self._verbose), self._pools, self._decoders,
+                          compute, on_short=too_short, on_error=self._decode_failed, group=self.GROUP)  # fmt: skip
 
     @staticmethod
     def _decode_failed(clip, e) -> None:

@@ -129,6 +129,13 @@ int cb_resize_cubic_u8(cb_ctx* ctx, const cb_surface_pool* pool, const int32_t* 
  * null, not both. */
 int cb_video_tube(cb_ctx* ctx, const cb_surface_pool* pool, const int32_t* slots, int n, int out_w, int out_h, const float mean[3],
                   const float std_[3], float* out_f32, uint8_t* out_u8, void* stream);
+/* cb_video_tube at size x size written straight as the InternVideo2 tower's patch rows: out_f16 [n][(size / patch)^2][k_pad], k = (c, y, x)
+ * of the patch, columns 3 patch^2 .. k_pad - 1 written as zeros.  Each value is the fp16 rounding (round to nearest even) of the fp32
+ * value cb_video_tube gives, so this equals cb_tube_patches(cb_video_tube(...)) bit for bit.  Replaces _construct_frames
+ * (models/internvideo2_mm.py:390-405) and the PatchEmbed input of the tower (internvideo2.py PatchEmbed, the Conv3d's im2col) in one
+ * launch.  k_pad even and >= 3 patch^2, size >= patch; n == 0 is a no-op. */
+int cb_video_tube_patches(cb_ctx* ctx, const cb_surface_pool* pool, const int32_t* slots, int n, int size, int patch, int k_pad, const float mean[3],
+                          const float std_[3], void* out_f16, void* stream);
 
 /* Full-resolution NV12 -> RGB24 (HWC, tightly packed): what decode_video_cpu_frame_ids returns per
  * frame (decoder_utils.py:439-451) / cvcuda.cvtcolor_into (nvcodec_utils.py:178).  Only for callers that
@@ -376,6 +383,12 @@ int cb_iv2_finalize(cb_iv2* iv2, int max_clips);
 /* tubes: device fp32 [n][frames][3][image_size][image_size] (InternVideo2FrameCreationStage's tubes); emb_out: device fp32
  * [n][embed_dim], unit norm.  Clips are independent: an embedding does not depend on the other clips of the call. */
 int cb_iv2_forward(cb_iv2* iv2, const float* tubes, int n, float* emb_out, void* stream);
+/* Decoded frames to clip embeddings in one call: slots holds n_clips * frames surface indices of `pool`, clip-major (any order, repeats
+ * allowed); each chunk of up to max_clips clips is one cb_video_tube_patches launch at image_size into the workspace, then the tower from
+ * the patch GEMM on.  emb_out: device fp32 [n_clips][embed_dim], bitwise what cb_iv2_forward gives for cb_video_tube's tubes of the same
+ * frames.  The pool's frame size is free (the frames are resized).  CB_ERR_STATE before finalize, n_clips == 0 is a no-op. */
+int cb_iv2_embed_surfaces(cb_iv2* iv2, const cb_surface_pool* pool, const int32_t* slots, int n_clips, const float mean[3], const float std_[3],
+                          float* emb_out, void* stream);
 
 /* ---- InternVideo2 text tower (text embeddings) ------------------------------------------------------- */
 /* InternVideo2_Stage2.get_txt_feat (models/internvideo2_mm.py:219-241) after tokenization: BertModel(mode="text") (bert/xbert.py), i.e.
