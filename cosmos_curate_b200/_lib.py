@@ -24,6 +24,8 @@ ARCH_CLIP, ARCH_SIGLIP = 0, 1
 EPI_NONE, EPI_QUICK_GELU, EPI_GELU_TANH, EPI_GELU_ERF = 0, 1, 2, 3
 DECODE_SEEK_SYNC, DECODE_DISCARD_ALL = 1, 2
 CUBIC_OPENCV, CUBIC_IPP = 0, 1
+PRE_NONE, PRE_TC, PRE_SIMT = 0, 1, 2
+PRE_WHY = ("OK", "RGB", "TAPS40", "KW", "RU", "UNITS", "SMEM", "TAPS64", "SWA", "ODD")  # CB_PRE_WHY_* by value
 
 
 class CurateB200Error(RuntimeError):
@@ -37,6 +39,19 @@ class SurfacePool(C.Structure):
         ("base", C.c_void_p), ("slot_stride", C.c_size_t), ("width", C.c_int), ("height", C.c_int),
         ("pitch", C.c_int), ("luma_rows", C.c_int), ("format", C.c_int),
     ]  # fmt: skip
+
+
+class PreprocessPlan(C.Structure):
+    """cb_preprocess_plan_info: the resample kernel and geometry cb_preprocess_clip would use."""
+
+    _fields_ = [(name, C.c_int) for name in (
+        "kernel", "simt_kernel", "tc_why", "simt_why", "new_w", "new_h", "top", "left", "taps_x", "taps_y", "src_y_begin", "src_y_end",
+        "tc_nc", "tc_n_slabs", "tc_kw", "tc_kb", "tc_ru", "tc_n_units", "tc_y_begin", "tc_smem",
+        "simt_tc", "simt_tiles", "simt_swa", "simt_gu", "simt_ring", "simt_n_strips", "simt_y_begin", "simt_smem",
+    )]  # fmt: skip
+
+    def as_dict(self) -> dict:
+        return {name: getattr(self, name) for name, _ in self._fields_}
 
 
 class VitCfg(C.Structure):
@@ -90,6 +105,7 @@ SIGNATURES = {
     "cb_profile_end": (_i, [_vp, _vp, _pf, C.POINTER(_i), _i]),
     "cb_preprocess_clip": (_i, [_vp, C.POINTER(SurfacePool), _pi32, _i, _i, _i, _i, _i, _i, _pf, _pf, _vp, _vp]),
     "cb_preprocess_clip_u8": (_i, [_vp, C.POINTER(SurfacePool), _pi32, _i, _i, _vp, _vp]),
+    "cb_preprocess_plan": (_i, [_vp, _i, _i, _i, _i, C.POINTER(PreprocessPlan)]),
     "cb_preprocess_bilinear_u8": (_i, [_vp, C.POINTER(SurfacePool), _pi32, _i, _i, _i, _vp, _vp]),
     "cb_resize_cubic_u8": (_i, [_vp, C.POINTER(SurfacePool), _pi32, _i, _i, _i, _i, _vp, _vp]),
     "cb_video_tube": (_i, [_vp, C.POINTER(SurfacePool), _pi32, _i, _i, _i, _pf, _pf, _vp, _vp, _vp]),

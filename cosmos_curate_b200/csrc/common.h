@@ -80,6 +80,16 @@ int make_tensor_map(cb_ctx* ctx, CUtensorMap* out, CUtensorMapDataType dtype, in
                     const uint64_t* strides_bytes /* rank-1 */, const uint32_t* box, CUtensorMapSwizzle swizzle);
 
 const TapTable* get_taps(cb_ctx* ctx, int in_size, int out_size, int crop_off, int crop_len);
+// The host half of get_taps: h_min, h_size, h_w, max_taps and the source range of one axis; allocates nothing.
+void compute_taps(int in_size, int out_size, int crop_off, int crop_len, TapTable* t);
+// preprocess_tc.cu: the tensor-pipe kernel's geometry for a request (host only, allocates nothing).  why is CB_PRE_WHY_OK when the kernel
+// serves it, else the first limit it breaks (CB_PRE_WHY_KW, _RU, _UNITS, _SMEM).
+struct TcGeometry {
+  int nc = 0, n_slabs = 0, kw = 0, kb = 0, ru = 0, n_units = 0, y_begin = 0, why = 0;
+  size_t smem = 0;
+  std::vector<int> x_lo, k0, nk;  // [n_slabs] window start, [n_slabs * 2] first k-step and k-steps of each N-tile
+};
+void tc_geometry(const TapTable& tx, const TapTable& ty, int res, TcGeometry* g);
 // preprocess_tc.cu: tensor-pipe resample into u8 [n][3][res][res] (returns CB_OK, 1 = configuration not served -> use the SIMT kernel,
 // < 0 = error)
 int run_clip_preprocess_tc(cb_ctx* ctx, const cb_surface_pool* pool, const int* d_slots, int n, int max_slot, int res, const TapTable* tx,

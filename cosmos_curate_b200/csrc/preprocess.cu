@@ -580,11 +580,8 @@ static float cubic_aa(float x) {  // Keys a = -0.5, float32 like ATen's bicubic_
   return 0.f;
 }
 
-const TapTable* get_taps(cb_ctx* ctx, int in_size, int out_size, int crop_off, int crop_len) {
-  auto key = std::make_tuple(in_size, out_size, crop_off, crop_len);
-  auto it = ctx->taps.find(key);
-  if (it != ctx->taps.end()) return &it->second;
-  TapTable t;
+void compute_taps(int in_size, int out_size, int crop_off, int crop_len, TapTable* tp) {
+  TapTable& t = *tp;
   t.in_size = in_size, t.out_size = out_size, t.crop_off = crop_off, t.crop_len = crop_len;
   // ATen upsample_antialias::_compute_weights_span / _compute_weights in float32
   volatile float scale = (float)in_size / (float)out_size;
@@ -617,15 +614,23 @@ const TapTable* get_taps(cb_ctx* ctx, int in_size, int out_size, int crop_off, i
     t.src_begin = std::min(t.src_begin, xmin);
     t.src_end = std::max(t.src_end, xmin + xsize);
   }
-  std::vector<float> flat((size_t)crop_len * t.max_taps, 0.f);
-  for (int o = 0; o < crop_len; ++o) std::copy(w[o].begin(), w[o].end(), flat.begin() + (size_t)o * t.max_taps);
+  t.h_w.assign((size_t)crop_len * t.max_taps, 0.f);
+  for (int o = 0; o < crop_len; ++o) std::copy(w[o].begin(), w[o].end(), t.h_w.begin() + (size_t)o * t.max_taps);
+}
+
+const TapTable* get_taps(cb_ctx* ctx, int in_size, int out_size, int crop_off, int crop_len) {
+  auto key = std::make_tuple(in_size, out_size, crop_off, crop_len);
+  auto it = ctx->taps.find(key);
+  if (it != ctx->taps.end()) return &it->second;
+  TapTable t;
+  compute_taps(in_size, out_size, crop_off, crop_len, &t);
+  const std::vector<float>& flat = t.h_w;
   if (cudaMalloc(&t.d_min, crop_len * sizeof(int)) != cudaSuccess || cudaMalloc(&t.d_size, crop_len * sizeof(int)) != cudaSuccess ||
       cudaMalloc(&t.d_w, flat.size() * sizeof(float)) != cudaSuccess)
     return nullptr;
   cudaMemcpy(t.d_min, t.h_min.data(), crop_len * sizeof(int), cudaMemcpyHostToDevice);
   cudaMemcpy(t.d_size, t.h_size.data(), crop_len * sizeof(int), cudaMemcpyHostToDevice);
   cudaMemcpy(t.d_w, flat.data(), flat.size() * sizeof(float), cudaMemcpyHostToDevice);
-  t.h_w = flat;
   auto res = ctx->taps.emplace(key, std::move(t));
   return &res.first->second;
 }
@@ -650,6 +655,13 @@ int ensure_norm_lut(cb_ctx* ctx, const float mean[3], const float std_[3], cudaS
 }
 
 static int python_round_half_even(double v) { return (int)std::nearbyint(v); }  // default FE_TONEAREST
+
+// torchvision Resize(res) + CenterCrop(res): short side -> res, long side -> int(res * long / short); crop offsets round half even
+static void resize_crop(int W, int H, int res, int* new_w, int* new_h, int* top, int* left) {
+  if (W <= H) *new_w = res, *new_h = (int)((long long)res * H / W);
+  else *new_h = res, *new_w = (int)((long long)res * W / H);
+  *top = python_round_half_even((*new_h - res) / 2.0), *left = python_round_half_even((*new_w - res) / 2.0);
+}
 
 static int upload_slots(cb_ctx* ctx, const int32_t* slots, int n, cudaStream_t stream, const int** out) {
   if (ctx->slots_cap < n) {
@@ -678,33 +690,33 @@ static int check_pool(cb_ctx* ctx, const cb_surface_pool* pool, int n, const int
   return CB_OK;
 }
 
-// SIMT kernel: column tiles, tensor maps and launch, into u8 `out` [n][3][res][res].  run_clip_preprocess has checked the request,
-// built the tap tables and uploaded the slots.
-static int run_clip_preprocess_simt(cb_ctx* ctx, const cb_surface_pool* pool, const int* d_slots, int n, int max_slot, int res, const TapTable* tx,
-                                    const TapTable* ty, uint8_t* out, cudaStream_t stream) {
-  const int W = pool->width, H = pool->height;
-  ClipArgs a{};
-  a.slots = d_slots, a.n = n, a.src_w = W, a.src_h = H, a.res = res;
-  a.xmin = tx->d_min, a.xsize = tx->d_size, a.wx = tx->d_w, a.tx = tx->max_taps;
-  a.ymin = ty->d_min, a.ysize = ty->d_size, a.wy = ty->d_w, a.ty = ty->max_taps;
-  a.out = out;
-  a.y_begin = ty->src_begin & ~1;
-  a.n_strips = (ty->src_end - a.y_begin + kSR - 1) / kSR;
+// The SIMT kernel's geometry for a request: column tile, strip window, union window, ring and shared memory.  Host only, allocates
+// nothing: run_clip_preprocess_simt launches from it and cb_preprocess_plan reports it.  why is CB_PRE_WHY_OK when the kernel serves
+// the request, else CB_PRE_WHY_SWA or CB_PRE_WHY_SMEM.
+struct SimtGeometry {
+  int tc = 0, tiles = 0, swa = 0, gu = 0, ring = 0, n_strips = 0, y_begin = 0, x_align = 16, why = 0;
+  size_t smem = 0;
+};
+
+static void simt_geometry(const TapTable& tx, const TapTable& ty, int res, int format, SimtGeometry* g) {
+  SimtGeometry& a = *g;
+  a.y_begin = ty.src_begin & ~1;
+  a.n_strips = (ty.src_end - a.y_begin + kSR - 1) / kSR;
   int ring = 64;
-  while (ring < kSR + ty->max_taps) ring <<= 1;
+  while (ring < kSR + ty.max_taps) ring <<= 1;
   a.ring = ring;
   a.x_align = 16;  // cp.async.bulk.tensor needs the box to start on a 16-byte boundary of the innermost dimension
   // widest source span of any column tile; strong downscales (4K -> 224: 9.6 source pixels per output column) narrow the tile
   // (32 -> 16 -> 8 columns) so that the window still fits one TMA box (256 bytes of the innermost dimension).  Under the 64-tap limit
   // an 8-column window spans at most ~200 source columns.
-  int span = 0, tiles = 0;
+  int span = 0;
   for (a.tc = 32;; a.tc /= 2) {
     span = 0;
-    tiles = (res + a.tc - 1) / a.tc;
-    for (int t = 0; t < tiles; ++t) {
+    a.tiles = (res + a.tc - 1) / a.tc;
+    for (int t = 0; t < a.tiles; ++t) {
       const int c0 = t * a.tc, c1 = std::min(res, c0 + a.tc);
-      int lo = tx->h_min[c0] & ~(a.x_align - 1), hi = 0;
-      for (int c = c0; c < c1; ++c) hi = std::max(hi, tx->h_min[c] + tx->h_size[c]);
+      int lo = tx.h_min[c0] & ~(a.x_align - 1), hi = 0;
+      for (int c = c0; c < c1; ++c) hi = std::max(hi, tx.h_min[c] + tx.h_size[c]);
       span = std::max(span, hi - lo);
     }
     if (span <= 256 || a.tc == 8) break;
@@ -716,11 +728,35 @@ static int run_clip_preprocess_simt(cb_ctx* ctx, const cb_surface_pool* pool, co
     if ((c % a.tc) + 4 > a.tc && (c % a.tc) % 4) continue;
     const int cl = std::min(res, std::min(c + 4, (c / a.tc + 1) * a.tc));
     int hi = 0;
-    for (int k = c; k < cl; ++k) hi = std::max(hi, tx->h_min[k] + tx->h_size[k] - tx->h_min[c]);
+    for (int k = c; k < cl; ++k) hi = std::max(hi, tx.h_min[k] + tx.h_size[k] - tx.h_min[c]);
     gu = std::max(gu, hi);
   }
   a.gu = gu;
-  if (a.swa > 256) return fail(ctx, CB_ERR_UNSUPPORTED, "downscale too large for one TMA box (%d source columns per tile)", a.swa);
+  const int raw_stage = is_nv12(format) ? (a.swa * kSR * 3 / 2) : (3 * a.swa * kSR);
+  const int groups = (a.tc + 3) / 4;
+  // the kernel's carve-up in order; 80 bytes cover the two mbarriers and the alignment of the weight table and the barriers
+  a.smem = 2 * (size_t)raw_stage + (size_t)3 * kSR * (a.swa + 1) * 4 + (size_t)3 * a.ring * (a.tc | 1) * 4 + (size_t)groups * a.gu * 16 +
+           (size_t)2 * groups * 4 + 80;
+  a.why = a.swa > 256 ? CB_PRE_WHY_SWA : a.smem > 227 * 1024 ? CB_PRE_WHY_SMEM : CB_PRE_WHY_OK;
+}
+
+// SIMT kernel: column tiles, tensor maps and launch, into u8 `out` [n][3][res][res].  run_clip_preprocess has checked the request,
+// built the tap tables and uploaded the slots.
+static int run_clip_preprocess_simt(cb_ctx* ctx, const cb_surface_pool* pool, const int* d_slots, int n, int max_slot, int res, const TapTable* tx,
+                                    const TapTable* ty, uint8_t* out, cudaStream_t stream) {
+  const int W = pool->width, H = pool->height;
+  SimtGeometry g;
+  simt_geometry(*tx, *ty, res, pool->format, &g);
+  if (g.why == CB_PRE_WHY_SWA) return fail(ctx, CB_ERR_UNSUPPORTED, "downscale too large for one TMA box (%d source columns per tile)", g.swa);
+  if (g.why != CB_PRE_WHY_OK) return fail(ctx, CB_ERR_UNSUPPORTED, "preprocess tile needs %zu bytes of shared memory", g.smem);
+  ClipArgs a{};
+  a.slots = d_slots, a.n = n, a.src_w = W, a.src_h = H, a.res = res;
+  a.xmin = tx->d_min, a.xsize = tx->d_size, a.wx = tx->d_w, a.tx = tx->max_taps;
+  a.ymin = ty->d_min, a.ysize = ty->d_size, a.wy = ty->d_w, a.ty = ty->max_taps;
+  a.out = out;
+  a.y_begin = g.y_begin, a.n_strips = g.n_strips, a.ring = g.ring, a.x_align = g.x_align, a.tc = g.tc, a.swa = g.swa, a.gu = g.gu;
+  const int tiles = g.tiles;
+  const size_t smem = g.smem;
   CUtensorMap map_a, map_b;
   int rc;
   if (is_nv12(pool->format)) {
@@ -743,12 +779,6 @@ static int run_clip_preprocess_simt(cb_ctx* ctx, const cb_surface_pool* pool, co
     map_b = map_a;
   }
 
-  const int raw_stage = is_nv12(pool->format) ? (a.swa * kSR * 3 / 2) : (3 * a.swa * kSR);
-  const int groups = (a.tc + 3) / 4;
-  // the kernel's carve-up in order; 80 bytes cover the two mbarriers and the alignment of the weight table and the barriers
-  const size_t smem = 2 * (size_t)raw_stage + (size_t)3 * kSR * (a.swa + 1) * 4 + (size_t)3 * a.ring * (a.tc | 1) * 4 + (size_t)groups * a.gu * 16 +
-                      (size_t)2 * groups * 4 + 80;
-  if (smem > 227 * 1024) return fail(ctx, CB_ERR_UNSUPPORTED, "preprocess tile needs %zu bytes of shared memory", smem);
   const auto kernel = pool->format == CB_FMT_NV12       ? clip_preprocess_simt_kernel<CB_FMT_NV12>
                       : pool->format == CB_FMT_NV12_SWS ? clip_preprocess_simt_kernel<CB_FMT_NV12_SWS>
                                                         : clip_preprocess_simt_kernel<CB_FMT_RGB24>;
@@ -773,14 +803,10 @@ int run_clip_preprocess(cb_ctx* ctx, const cb_surface_pool* pool, const int32_t*
   if (((uintptr_t)pool->base & 15) || (pool->pitch & 15) || (pool->slot_stride & 15))
     return fail(ctx, CB_ERR_ARG, "TMA needs base/pitch/slot_stride multiples of 16 bytes");
   if (is_nv12(pool->format) && ((pool->width | pool->height) & 1)) return fail(ctx, CB_ERR_UNSUPPORTED, "NV12 needs even dimensions");
-  const int W = pool->width, H = pool->height;
-  // torchvision: short side -> res, long side -> int(res * long / short); centre crop res x res
-  int new_w, new_h;
-  if (W <= H) new_w = res, new_h = (int)((long long)res * H / W);
-  else new_h = res, new_w = (int)((long long)res * W / H);
-  const int top = python_round_half_even((new_h - res) / 2.0), left = python_round_half_even((new_w - res) / 2.0);
-  const TapTable* tx = get_taps(ctx, W, new_w, left, res);
-  const TapTable* ty = get_taps(ctx, H, new_h, top, res);
+  int new_w, new_h, top, left;
+  resize_crop(pool->width, pool->height, res, &new_w, &new_h, &top, &left);
+  const TapTable* tx = get_taps(ctx, pool->width, new_w, left, res);
+  const TapTable* ty = get_taps(ctx, pool->height, new_h, top, res);
   if (!tx || !ty) return fail(ctx, CB_ERR_CUDA, "tap table allocation failed");
   if (out_mode == 2) {
     if (layout_patch <= 0 || layout_patch > 32 || res < layout_patch) return fail(ctx, CB_ERR_UNSUPPORTED, "patch %d unsupported for res %d", layout_patch, res);
@@ -826,6 +852,42 @@ int run_clip_preprocess(cb_ctx* ctx, const cb_surface_pool* pool, const int32_t*
     pack_patches_kernel<<<dim3(res / layout_patch, n), 256, kz * sizeof(int), stream>>>(q);
   }
   CB_CUDA(ctx, cudaGetLastError());
+  return CB_OK;
+}
+
+// cb_preprocess_plan: the decisions of run_clip_preprocess, run_clip_preprocess_tc and run_clip_preprocess_simt from the same host
+// functions, without tap tables on the device or a launch.
+static int preprocess_plan(cb_ctx* ctx, int W, int H, int format, int res, cb_preprocess_plan_info* o) {
+  if (!o) return fail(ctx, CB_ERR_ARG, "null plan output");
+  if (!is_nv12(format) && format != CB_FMT_RGB24) return fail(ctx, CB_ERR_ARG, "unknown surface format %d", format);
+  if (W <= 0 || H <= 0) return fail(ctx, CB_ERR_ARG, "bad surface size %dx%d", W, H);
+  if (res <= 0 || res > 1024) return fail(ctx, CB_ERR_ARG, "bad output resolution %d", res);
+  *o = cb_preprocess_plan_info{};
+  resize_crop(W, H, res, &o->new_w, &o->new_h, &o->top, &o->left);
+  if (is_nv12(format) && ((W | H) & 1)) {
+    o->kernel = o->simt_kernel = CB_PRE_NONE, o->tc_why = o->simt_why = CB_PRE_WHY_ODD;
+    return CB_OK;
+  }
+  TapTable tx, ty;
+  compute_taps(W, o->new_w, o->left, res, &tx);
+  compute_taps(H, o->new_h, o->top, res, &ty);
+  o->taps_x = tx.max_taps, o->taps_y = ty.max_taps, o->src_y_begin = ty.src_begin, o->src_y_end = ty.src_end;
+  if (tx.max_taps > 64 || ty.max_taps > 64) {
+    o->kernel = o->simt_kernel = CB_PRE_NONE, o->tc_why = o->simt_why = CB_PRE_WHY_TAPS64;
+    return CB_OK;
+  }
+  TcGeometry t;
+  tc_geometry(tx, ty, res, &t);
+  o->tc_nc = t.nc, o->tc_n_slabs = t.n_slabs, o->tc_kw = t.kw, o->tc_kb = t.kb, o->tc_ru = t.ru, o->tc_n_units = t.n_units;
+  o->tc_y_begin = t.y_begin, o->tc_smem = (int)t.smem;
+  o->tc_why = !is_nv12(format) ? CB_PRE_WHY_RGB : ty.max_taps > 40 ? CB_PRE_WHY_TAPS40 : t.why;
+  SimtGeometry g;
+  simt_geometry(tx, ty, res, format, &g);
+  o->simt_tc = g.tc, o->simt_tiles = g.tiles, o->simt_swa = g.swa, o->simt_gu = g.gu, o->simt_ring = g.ring, o->simt_n_strips = g.n_strips;
+  o->simt_y_begin = g.y_begin, o->simt_smem = (int)g.smem;
+  o->simt_why = g.why;
+  o->simt_kernel = g.why == CB_PRE_WHY_OK ? CB_PRE_SIMT : CB_PRE_NONE;
+  o->kernel = o->tc_why == CB_PRE_WHY_OK ? CB_PRE_TC : o->simt_kernel;
   return CB_OK;
 }
 
@@ -1025,6 +1087,10 @@ int cb_preprocess_clip_u8(cb_ctx* ctx, const cb_surface_pool* pool, const int32_
   if (!ctx) return CB_ERR_ARG;
   const float m[3] = {0, 0, 0}, s[3] = {1, 1, 1};
   return cb::run_clip_preprocess(ctx, pool, slots, n, res, 0, 0, 0, CB_DT_F32, m, s, out, (cudaStream_t)stream);
+}
+
+int cb_preprocess_plan(cb_ctx* ctx, int width, int height, int format, int res, cb_preprocess_plan_info* out) {
+  return cb::preprocess_plan(ctx, width, height, format, res, out);
 }
 
 int cb_preprocess_bilinear_u8(cb_ctx* ctx, const cb_surface_pool* pool, const int32_t* slots, int n, int out_w, int out_h, uint8_t* out,

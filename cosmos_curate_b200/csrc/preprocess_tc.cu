@@ -283,6 +283,7 @@ namespace {
 
 struct TcPlan {  // per (source size, taps): slab windows + pre-swizzled weight tiles on the device
   int n_slabs = 0, kw = 0, kb = 0, ru = 0, n_units = 0, y_begin = 0, nc = kNC;
+  size_t smem = 0;
   int *d_x_lo = nullptr, *d_k0 = nullptr, *d_nk = nullptr, *d_unit_last = nullptr;
   uint8_t* d_w = nullptr;
   bool ok = false;
@@ -307,44 +308,61 @@ static std::map<std::tuple<const TapTable*, const TapTable*>, TcPlan>& plans(cb_
   return all[ctx];
 }
 
-static const TcPlan* get_plan(cb_ctx* ctx, const TapTable* tx, const TapTable* ty, int res) {
-  auto key = std::make_tuple(tx, ty);
-  auto& cache = plans(ctx);
-  auto it = cache.find(key);
-  if (it != cache.end()) return &it->second;
-  TcPlan p;
-  std::vector<int> x_lo, k0, nk;
+// The tensor-pipe geometry of a request: 32-column slabs unless their source window exceeds one TMA box (4K -> 224: 9.6x downscale),
+// then 16; the N-tiles' k-step windows; rows per unit and units per frame column; shared memory.  Host only, allocates nothing:
+// get_plan builds the launch from it and cb_preprocess_plan reports it.
+void tc_geometry(const TapTable& tx, const TapTable& ty, int res, TcGeometry* g) {
+  TcGeometry& p = *g;
   int kw = 0, kbmax = 0;
-  for (int nc : {kNC, 16}) {  // 32 columns per slab unless their source window exceeds one TMA box (4K -> 224: 9.6x downscale)
+  for (int nc : {kNC, 16}) {
     p.nc = nc, p.n_slabs = (res + nc - 1) / nc;
-    x_lo.assign(p.n_slabs, 0), k0.assign(p.n_slabs * 2, 0), nk.assign(p.n_slabs * 2, 0);
+    p.x_lo.assign(p.n_slabs, 0), p.k0.assign(p.n_slabs * 2, 0), p.nk.assign(p.n_slabs * 2, 0);
     kw = 0, kbmax = 0;
     for (int s = 0; s < p.n_slabs; ++s) {
       const int c0 = s * nc, c1 = std::min(res, c0 + nc);
-      x_lo[s] = tx->h_min[c0] & ~15;
+      p.x_lo[s] = tx.h_min[c0] & ~15;
       int hi = 0;
-      for (int c = c0; c < c1; ++c) hi = std::max(hi, tx->h_min[c] + tx->h_size[c]);
-      kw = std::max(kw, hi - x_lo[s]);
+      for (int c = c0; c < c1; ++c) hi = std::max(hi, tx.h_min[c] + tx.h_size[c]);
+      kw = std::max(kw, hi - p.x_lo[s]);
       for (int j = 0; j < 2; ++j) {
         const int t0 = c0 + 16 * j, t1 = std::min(c1, t0 + 16);
         if (t0 >= t1) continue;
-        const int first = (tx->h_min[t0] - x_lo[s]) / 16;
+        const int first = (tx.h_min[t0] - p.x_lo[s]) / 16;
         int end = 0;
-        for (int c = t0; c < t1; ++c) end = std::max(end, tx->h_min[c] + tx->h_size[c] - x_lo[s]);
-        k0[s * 2 + j] = first, nk[s * 2 + j] = (end - first * 16 + 15) / 16;
-        kbmax = std::max(kbmax, nk[s * 2 + j] * 16);
+        for (int c = t0; c < t1; ++c) end = std::max(end, tx.h_min[c] + tx.h_size[c] - p.x_lo[s]);
+        p.k0[s * 2 + j] = first, p.nk[s * 2 + j] = (end - first * 16 + 15) / 16;
+        kbmax = std::max(kbmax, p.nk[s * 2 + j] * 16);
       }
     }
     if (kw <= 256) break;
   }
   p.kw = (kw + 63) & ~63, p.kb = (kbmax + 63) & ~63;
-  p.ru = std::min(40, kRingRows - ty->max_taps + 1) & ~7;  // multiple of 8: a colour plane is a whole number of 8-row operand groups
-  p.y_begin = ty->src_begin & ~1;
-  p.n_units = p.ru > 0 ? (ty->src_end - p.y_begin + p.ru - 1) / p.ru : 0;
+  p.ru = std::min(40, kRingRows - ty.max_taps + 1) & ~7;  // multiple of 8: a colour plane is a whole number of 8-row operand groups
+  p.y_begin = ty.src_begin & ~1;
+  p.n_units = p.ru > 0 ? (ty.src_end - p.y_begin + p.ru - 1) / p.ru : 0;
   const int b_tile = (p.kb / 64) * 4096;
-  const size_t smem = 1024 + (size_t)p.kw * 256 + 2 * (size_t)b_tile + ((((size_t)(p.ru + p.ru / 2) * p.kw) + 127) & ~(size_t)127) + (kRingRows * kRingStride + kVRows * kVTaps + 2 * kVRows + kMaxUnits) * 4 + 64;
-  p.ok = p.ru >= 16 && p.kw <= 256 && p.n_units <= kMaxUnits && smem <= 227 * 1024;  // TMA box <= 256 columns
+  p.smem = 1024 + (size_t)p.kw * 256 + 2 * (size_t)b_tile + ((((size_t)(p.ru + p.ru / 2) * p.kw) + 127) & ~(size_t)127) +
+           (kRingRows * kRingStride + kVRows * kVTaps + 2 * kVRows + kMaxUnits) * 4 + 64;
+  p.why = p.kw > 256                ? CB_PRE_WHY_KW  // TMA box <= 256 columns
+          : p.ru < 16               ? CB_PRE_WHY_RU
+          : p.n_units > kMaxUnits   ? CB_PRE_WHY_UNITS
+          : p.smem > 227 * 1024     ? CB_PRE_WHY_SMEM
+                                    : CB_PRE_WHY_OK;
+}
+
+static const TcPlan* get_plan(cb_ctx* ctx, const TapTable* tx, const TapTable* ty, int res) {
+  auto key = std::make_tuple(tx, ty);
+  auto& cache = plans(ctx);
+  auto it = cache.find(key);
+  if (it != cache.end()) return &it->second;
+  TcGeometry g;
+  tc_geometry(*tx, *ty, res, &g);
+  TcPlan p;
+  p.nc = g.nc, p.n_slabs = g.n_slabs, p.kw = g.kw, p.kb = g.kb, p.ru = g.ru, p.n_units = g.n_units, p.y_begin = g.y_begin, p.smem = g.smem;
+  p.ok = g.why == CB_PRE_WHY_OK;
+  const std::vector<int>&x_lo = g.x_lo, &k0 = g.k0, &nk = g.nk;
   if (p.ok) {
+    const int b_tile = (p.kb / 64) * 4096;
     std::vector<uint16_t> w((size_t)p.n_slabs * 2 * b_tile / 2, 0);
     for (int s = 0; s < p.n_slabs; ++s)
       for (int j = 0; j < 2; ++j)
@@ -418,11 +436,9 @@ int run_clip_preprocess_tc(cb_ctx* ctx, const cb_surface_pool* pool, const int* 
   a.colour = pool->format;
   a.x_lo = p->d_x_lo, a.tile_k0 = p->d_k0, a.tile_nk = p->d_nk, a.wtiles = p->d_w;
   a.ymin = ty->d_min, a.ysize = ty->d_size, a.unit_last = p->d_unit_last, a.wy = ty->d_w, a.ty = ty->max_taps, a.out = out;
-  const int b_tile = (p->kb / 64) * 4096;
-  const size_t smem = 1024 + (size_t)p->kw * 256 + 2 * (size_t)b_tile + ((((size_t)(p->ru + p->ru / 2) * p->kw) + 127) & ~(size_t)127) + (kRingRows * kRingStride + kVRows * kVTaps + 2 * kVRows + kMaxUnits) * 4 + 64;
-  CB_CUDA(ctx, cudaFuncSetAttribute(clip_preprocess_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  CB_CUDA(ctx, cudaFuncSetAttribute(clip_preprocess_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)p->smem));
   mark_launch(ctx, CB_PROF_PREPROCESS, stream);
-  clip_preprocess_tc_kernel<<<dim3(p->n_slabs, n), kTcThreads, smem, stream>>>(map_y, map_uv, a);
+  clip_preprocess_tc_kernel<<<dim3(p->n_slabs, n), kTcThreads, p->smem, stream>>>(map_y, map_uv, a);
   CB_CUDA(ctx, cudaGetLastError());
   return CB_OK;
 }

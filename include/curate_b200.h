@@ -105,6 +105,38 @@ int cb_preprocess_clip(cb_ctx* ctx, const cb_surface_pool* pool, const int32_t* 
 int cb_preprocess_clip_u8(cb_ctx* ctx, const cb_surface_pool* pool, const int32_t* slots, int n, int res, uint8_t* out,
                           void* stream);
 
+/* Which resample kernel cb_preprocess_clip / cb_preprocess_clip_u8 would run for a width x height pool of `format` at `res`, and
+ * its geometry.  Launches nothing, allocates nothing and reads no environment; ctx may be null (then errors carry no message).
+ * Returns CB_ERR_ARG for a null `out`, an unknown format, a size <= 0 or res outside 1..1024, else CB_OK with `out` filled: a
+ * request the library refuses with CB_ERR_UNSUPPORTED (odd NV12 size, more than 64 taps on an axis) has kernel = CB_PRE_NONE. */
+#define CB_PRE_NONE 0 /* the call returns CB_ERR_UNSUPPORTED */
+#define CB_PRE_TC 1   /* clip_preprocess_tc_kernel: horizontal pass on the tensor pipe (NV12 only) */
+#define CB_PRE_SIMT 2 /* clip_preprocess_simt_kernel */
+/* why a kernel does not serve a request (tc_why, simt_why) */
+#define CB_PRE_WHY_OK 0
+#define CB_PRE_WHY_RGB 1    /* tensor pipe: RGB pools */
+#define CB_PRE_WHY_TAPS40 2 /* tensor pipe: more than 40 vertical taps */
+#define CB_PRE_WHY_KW 3     /* tensor pipe: a 16-column slab's source window exceeds one 256-byte TMA box */
+#define CB_PRE_WHY_RU 4     /* tensor pipe: fewer than 16 source rows per unit */
+#define CB_PRE_WHY_UNITS 5  /* tensor pipe: more units per frame column than the kernel stages */
+#define CB_PRE_WHY_SMEM 6   /* more than 227 KB of shared memory */
+#define CB_PRE_WHY_TAPS64 7 /* more than 64 taps on either axis: neither kernel */
+#define CB_PRE_WHY_SWA 8    /* SIMT: an 8-column tile's source window exceeds one 256-byte TMA box */
+#define CB_PRE_WHY_ODD 9    /* NV12 with an odd width or height: neither kernel */
+typedef struct cb_preprocess_plan_info {
+  int kernel;          /* CB_PRE_*: what the default call runs */
+  int simt_kernel;     /* what the call runs with CB_PRE_KERNEL=simt: CB_PRE_SIMT or CB_PRE_NONE */
+  int tc_why, simt_why;                /* CB_PRE_WHY_* of each kernel */
+  int new_w, new_h, top, left;         /* Resize(res) output size (short side -> res) and CenterCrop(res) offsets */
+  int taps_x, taps_y;                  /* widest tap window of the cropped outputs per axis */
+  int src_y_begin, src_y_end;          /* source rows the cropped outputs tap */
+  /* tensor-pipe geometry; zero when taps_x or taps_y > 64 or the request is refused */
+  int tc_nc, tc_n_slabs, tc_kw, tc_kb, tc_ru, tc_n_units, tc_y_begin, tc_smem;
+  /* SIMT geometry; zero when taps_x or taps_y > 64 or the request is refused */
+  int simt_tc, simt_tiles, simt_swa, simt_gu, simt_ring, simt_n_strips, simt_y_begin, simt_smem;
+} cb_preprocess_plan_info;
+int cb_preprocess_plan(cb_ctx* ctx, int width, int height, int format, int res, cb_preprocess_plan_info* out);
+
 /* Fused NV12->RGB + bilinear resize to out_w x out_h, u8 HWC: out[n][out_h][out_w][3].  Replaces
  * cvcuda.cvtcolor_into + cvcuda.resize_into(Interp.LINEAR) (nvcodec_utils.py:178,189-194), the
  * 27x48 shot-detection frames of VideoFrameExtractionStage (frame_extraction_stages.py:112-116). */

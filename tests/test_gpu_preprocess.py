@@ -14,7 +14,7 @@ import pytest
 import torch
 
 from conftest import golden_json, load_golden
-from gpu_helpers import ctx, nv12_pool as _nv12_pool, u8_budget as _u8_budget  # noqa: F401
+from gpu_helpers import assert_typed_outputs_are_lut_of, ctx, nv12_pool as _nv12_pool, u8_budget as _u8_budget  # noqa: F401
 from oracle import color, preprocess, vit
 
 pytestmark = pytest.mark.gpu
@@ -191,22 +191,10 @@ def test_tensor_pipe_preprocess_agrees_with_simt_kernel_and_oracle(ctx, monkeypa
         for i, f in enumerate(frames):
             buf[i, :, :w] = f
         pool = ctx.nv12_pool(torch.from_numpy(buf).cuda(), w, h, h, colour=colour)
-    lut = preprocess.normalize_lut()
-
-    def assert_typed_outputs_are_lut_of(u8):
-        want32 = np.stack([lut[c][u8[:, c]] for c in range(3)], axis=1)
-        np.testing.assert_array_equal(ctx.preprocess_clip(pool, res=res, dtype=torch.float32).cpu().numpy(), want32)
-        for patch, k_pad in ((14, 640), (16, 768)):
-            gp = ctx.preprocess_clip(pool, res=res, dtype=torch.float16, layout="patch", patch=patch, k_pad=k_pad).cpu().numpy()
-            np.testing.assert_array_equal(gp, preprocess.to_patches(want32.astype(np.float16), patch, k_pad))
-            gb = ctx.preprocess_clip(pool, res=res, dtype=torch.bfloat16, layout="patch", patch=patch, k_pad=k_pad).float().cpu().numpy()
-            want_bf = torch.from_numpy(want32).to(torch.bfloat16).float().numpy()
-            np.testing.assert_array_equal(gb, preprocess.to_patches(want_bf, patch, k_pad))
-
     got_tc = ctx.preprocess_clip_u8(pool, res=res).cpu().numpy()
     monkeypatch.setenv("CB_PRE_KERNEL", "simt")
     got_simt = ctx.preprocess_clip_u8(pool, res=res).cpu().numpy()
-    assert_typed_outputs_are_lut_of(got_simt)
+    assert_typed_outputs_are_lut_of(ctx, pool, res, got_simt)
     monkeypatch.delenv("CB_PRE_KERNEL")
     want = preprocess.clip_resize_crop_u8(rgb, res)
     _u8_budget(got_tc, want)
@@ -214,7 +202,7 @@ def test_tensor_pipe_preprocess_agrees_with_simt_kernel_and_oracle(ctx, monkeypa
     _u8_budget(got_tc, got_simt, frac=2e-4)  # two fp32 summation orders apart
     if res == 192 or colour == "rgb":  # the default call ran the SIMT kernel too
         np.testing.assert_array_equal(got_tc, got_simt)
-    assert_typed_outputs_are_lut_of(got_tc)
+    assert_typed_outputs_are_lut_of(ctx, pool, res, got_tc)
 
 
 def test_clip_preprocess_4k_rgb_frames_strong_downscale(ctx):
