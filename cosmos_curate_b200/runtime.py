@@ -847,3 +847,84 @@ def collect_group(jobs) -> tuple[int, list]:
         except _lib.CurateB200Error as e:
             errs.append(e)
     return decoded, errs
+
+
+def run_decode_groups(items, plan, pools: SurfacePools, decoders, compute, *, on_error, max_frames: int, on_short=None, depth: int = 2,
+                      seek_keyframes: bool = False) -> tuple[int, int]:  # fmt: skip
+    """Decode the kept frames of clips [(clip, mp4 bytes)] into surface pools, group by group, and hand each group to `compute`.
+
+    plan(clip, data) gives (surface size, ascending frame ids to decode, slot of every kept frame relative to the clip's first slot).
+    It raises CurateB200Error / ValueError for a clip that goes to on_error(clip, e); a plan that can return None (too few frames)
+    needs on_short(clip).  A clip keeping more than `max_frames` frames goes to on_error; the others are grouped per surface size, in the
+    order sizes are first seen, each group filled with whole clips up to `max_frames` kept frames.  Group k is decoded by decoders()
+    (a DecoderPool) into pool k % depth (depth >= 2) of its size's ring while the groups before it compute.
+
+    compute(k, pool, ok, slots) gets the clips whose decode succeeded as [(clip, number of kept frames)] (the others go to on_error)
+    and their kept frames' surface indices, concatenated clip-major.  It queues the GPU work that reads the pool and returns None or
+    a finisher that writes the results onto the clips.  Per group k: wait for its decode, compute(k) and record an event, wait on
+    group k - 1's event, submit group k + depth - 1, run group k - 1's finisher.  The GPU has group k queued while the host writes
+    k - 1's results and submits decode, and since a size's groups are contiguous, the last reader of the pool that group
+    k + depth - 1 decodes into is group k - 1 at the latest.  -> (frames decoded, groups)."""
+    by_size: dict[tuple, list] = {}
+    for clip, data in items:
+        try:
+            planned = plan(clip, data)
+        except (_lib.CurateB200Error, ValueError) as e:
+            on_error(clip, e)
+            continue
+        if planned is None:
+            on_short(clip)
+            continue
+        size, ids, inverse = planned
+        if len(inverse) > max_frames:
+            on_error(clip, ValueError(f"{len(inverse)} kept frames exceed max_frames={max_frames}"))
+            continue
+        by_size.setdefault(size, []).append((clip, data, ids, inverse))
+    groups: list[tuple[tuple, list]] = []
+    for size, clips in by_size.items():
+        used = max_frames
+        for c in clips:
+            if used + len(c[3]) > max_frames:
+                groups.append((size, []))
+                used = 0
+            groups[-1][1].append(c)
+            used += len(c[3])
+    ring_pos: dict[tuple, int] = {}
+    pending: dict[int, tuple] = {}
+
+    def submit(k):
+        size, clips = groups[k]
+        r = ring_pos.get(size, 0)
+        ring_pos[size] = (r + 1) % depth
+        pool = pools.get(size, sum(len(ids) for _, _, ids, _ in clips), r)
+        pending[k] = pool, decoders().submit_group(pool, size, [(data, ids) for _, data, ids, _ in clips], seek_keyframes)
+
+    decoded, prev_event, prev_finisher = 0, None, None  # of group k - 1
+    for k in range(min(depth - 1, len(groups))):
+        submit(k)
+    for k, (_, clips) in enumerate(groups):
+        pool, jobs = pending.pop(k)
+        n, errs = collect_group(jobs)
+        decoded += n
+        ok, slots = [], []
+        for (clip, _, _, inverse), (first, _), err in zip(clips, jobs, errs):
+            if err is not None:
+                on_error(clip, err)
+                continue
+            ok.append((clip, len(inverse)))
+            slots.append(first + inverse)
+        finisher = compute(k, pool, ok, np.concatenate(slots).astype(np.int32)) if ok else None
+        event = torch.cuda.Event()
+        event.record(torch.cuda.current_stream())
+        if prev_event is not None:
+            prev_event.synchronize()
+        if k + depth - 1 < len(groups):
+            submit(k + depth - 1)
+        if prev_finisher is not None:
+            prev_finisher()
+        prev_event, prev_finisher = event, finisher
+    if prev_event is not None:
+        prev_event.synchronize()
+        if prev_finisher is not None:
+            prev_finisher()
+    return decoded, len(groups)

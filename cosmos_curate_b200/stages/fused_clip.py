@@ -11,10 +11,12 @@ stage that never materialises RGB frames.  Task mutations and the error conventi
     (optional) clip.openai_embedding = L2-normalised mean of the per-frame embeddings (SURVEY.md 8b: the reference has
     no pooling rule for frame embeddings; this documented choice fills the existing generic clip-embedding slot).
 
-Inside one `process_data` call the work is pipelined (this IS the product path bench.py times as `e2e`): the clips of
-tower batches k+1 and k+2 are being decoded by the persistent NVDEC sessions (DecoderPool: one session per worker thread,
-kept across calls, pinned to the GPU's NUMA node) while the SMs run preprocess + tower on batch k out of a three-deep ring
-of surface pools; scores / embeddings come back through pinned host buffers with one async copy per batch.
+Inside one `process_data` call the work is pipelined by runtime.run_decode_groups, the decode-group loop the InternVideo2 stages
+run too (this IS the product path bench.py times as `e2e`): the clips of tower batches k+1 and k+2 are being decoded by the
+persistent NVDEC sessions (DecoderPool: one session per worker thread, kept across calls, pinned to the GPU's NUMA node) while
+the SMs run preprocess + tower on batch k out of a three-deep ring of surface pools; scores / embeddings come back through
+pinned host buffers with one async copy per batch.  A batch holds whole clips of one resolution, at most max_batch frames; a
+clip that samples more frames than that fails like a clip that does not decode.
 """
 
 from __future__ import annotations
@@ -25,11 +27,10 @@ import numpy as np
 import torch
 
 from .. import sampling
-from .._lib import CurateB200Error
 from ..data_model import StageTimer
 from ..interfaces import CuratorStage, CuratorStageResource, ModelInterface
 from ..models.clip_aesthetics import CLIPAestheticScorer
-from ..runtime import DecoderPool, SurfacePools, check_colour, collect_group, even_size, get_context, mp4_index
+from ..runtime import DecoderPool, SurfacePools, check_colour, even_size, get_context, mp4_index, run_decode_groups
 
 try:
     from loguru import logger
@@ -132,46 +133,22 @@ class NvdecClipAestheticStage(CuratorStage):
             self._pools.clear()
 
     # ---- helpers ---------------------------------------------------------------------------------
-    def _plan_span(self, clip, video):
-        """Frames of the source video inside clip.span, re-timed from the clip start and sampled like a clip of its own."""
-        data = video.encoded_data.resolve() if video.encoded_data else None
-        if data is None:
-            logger.warning(f"Clip {clip.uuid}: source video has no encoded_data.")
-            clip.errors["encoded_data"] = "empty"
-            clip.aesthetic_score = -1.0
-            return None
-        try:
-            cached = self._video_index.get(id(video))
-            if cached is None or cached[0] is not data:
-                idx = mp4_index(data)
-                cached = self._video_index[id(video)] = (data, idx, sampling.timestamps_from_index(idx["pts"], idx["timescale"]))
-            _, idx, ts = cached
-            ids = sampling.span_frame_ids(ts, clip.span, self._target_fps)
-            return data, ids, even_size(idx["width"], idx["height"])
-        except (CurateB200Error, ValueError) as e:
-            logger.error(f"Error extracting frames from clip {clip.uuid}: {e}")
-            clip.errors["frame_extraction"] = "video_decode_failed"
-            clip.aesthetic_score = -1.0
-            return None
-
-    def _plan(self, clip, video=None):
-        """-> (data u8 array, frame ids expanded, (w, h)) or None (errors recorded on the clip)."""
-        if self._source == "video_span":
-            return self._plan_span(clip, video)
-        data = clip.encoded_data.resolve() if clip.encoded_data else None
-        if data is None:
-            logger.warning(f"Clip {clip.uuid} has no encoded_data.")
-            clip.errors["encoded_data"] = "empty"
-            clip.aesthetic_score = -1.0
-            return None
-        try:
+    def _plan(self, clip, data):
+        """-> (surface size, sampled frame ids with repeats, slot of each relative to the clip's first), or raises for an unreadable
+        container or a span that selects no frame.  source="video_span": the source video's frames inside clip.span, re-timed from
+        the clip start and sampled like a clip of its own."""
+        cached = self._video_index.get(id(data))  # the clips of a span-sourced video share its bytes: indexed once per call
+        if cached is None:  # an entry holds its bytes, so their id names no other object while it exists
             idx = mp4_index(data)
-            ts = sampling.timestamps_from_index(idx["pts"], idx["timescale"])
+            cached = self._video_index[id(data)] = (data, even_size(idx["width"], idx["height"]),
+                                                    sampling.timestamps_from_index(idx["pts"], idx["timescale"]))  # fmt: skip
+        _, size, ts = cached
+        if self._source == "video_span":
+            ids = sampling.span_frame_ids(ts, clip.span, self._target_fps)
+        else:
             ids, counts = sampling.frame_ids(ts, sampling.FrameExtractionPolicy.sequence, self._target_fps)
-            return data, np.repeat(ids, counts).astype(np.int32), even_size(idx["width"], idx["height"])
-        except (CurateB200Error, ValueError) as e:
-            self._decode_failed(clip, e)
-            return None
+            ids = np.repeat(ids, counts).astype(np.int32)
+        return size, ids, np.arange(len(ids), dtype=np.int32)
 
     def _decode_failed(self, clip, e) -> None:
         logger.error(f"Error extracting frames from clip {clip.uuid}: {e}")
@@ -190,99 +167,59 @@ class NvdecClipAestheticStage(CuratorStage):
             self._host.append((score, emb))
         return self._host[r]
 
-    def _make_batches(self, by_size):
-        """[(size, [(clip, data, ids)])]: whole clips, at most max_batch frames, one resolution per batch."""
-        batches = []
-        for size, clips in by_size.items():
-            batch, used = [], 0
-            for clip, data, ids in clips:
-                if len(ids) > self._max_batch:
-                    self._decode_failed(clip, ValueError(f"{len(ids)} sampled frames exceed max_batch={self._max_batch}"))
-                    continue
-                if used + len(ids) > self._max_batch:
-                    batches.append((size, batch))
-                    batch, used = [], 0
-                batch.append((clip, data, ids))
-                used += len(ids)
-            if batch:
-                batches.append((size, batch))
-        return batches
+    def _compute(self, k, pool, ok, slots):
+        """Preprocess + tower on batch k's decoded frames and the D2H copy of the results into ring slot k % RING, queued; -> the
+        finisher that writes each clip's reduced score and L2-normalised mean embedding."""
+        tower = self._model.tower
+        norm = {} if self._norm[0] is None else {"mean": self._norm[0], "std": self._norm[1]}
+        if self._target_res is not None:
+            th, tw = self._target_res
+            small = self._ctx.resize_cubic_u8(pool, tw, th, slots=slots, mode=self._cubic_mode)
+            emb, _, score = tower.embed_pool(self._ctx.rgb_pool(small), **norm)
+        else:
+            emb, _, score = tower.embed_pool(pool, slots=slots, **norm)
+        n = len(slots)
+        score_h, emb_h = self._host_buffers(k % self.RING)
+        if score_h is not None:
+            score_h[:n].copy_(score, non_blocking=True)
+        if emb_h is not None:
+            emb_h[:n].copy_(emb, non_blocking=True)
 
-    def _run_batches(self, batches) -> None:
-        """Decode of batches k+1, k+2 (NVDEC + host parsing threads) overlaps preprocess + tower of batch k (SMs)."""
-        seek, tower, stream = self._seek, self._model.tower, torch.cuda.current_stream()
-        ring_pos: dict[tuple[int, int], int] = {}
-        groups, inflight = {}, {}
-        decoded = 0
-
-        def submit(k):
-            size, items = batches[k]
-            r = ring_pos.get(size, 0)
-            ring_pos[size] = (r + 1) % self.RING
-            pool = self._pools.get(size, self._max_batch, r)
-            groups[k] = (pool, self._decode_pool.submit_group(pool, size, [(data, ids) for _, data, ids in items], seek))
-
-        def finalize(k):
-            """Batch k's results are on the host once its event has fired: write them onto the clips."""
-            ev, jobs, errs, n = inflight.pop(k)
-            ev.synchronize()
-            score_h, emb_h = self._host_buffers(k % self.RING)
-            score_h = score_h[:n].numpy() if score_h is not None else None
-            for (clip, _, ids), (first, _), err in zip(batches[k][1], jobs, errs):
-                if err is not None:
-                    self._decode_failed(clip, err)
-                    continue
+        def write():
+            row = 0
+            for clip, m in ok:
                 if score_h is not None:
-                    clip.aesthetic_score = float(self._reduce_fn(score_h[first : first + len(ids)]))
+                    clip.aesthetic_score = float(self._reduce_fn(score_h[row : row + m].numpy()))
                 if emb_h is not None:
-                    m = emb_h[first : first + len(ids)].numpy().mean(axis=0)
-                    clip.openai_embedding = (m / np.linalg.norm(m)).astype(np.float32)
+                    e = emb_h[row : row + m].numpy().mean(axis=0)
+                    clip.openai_embedding = (e / np.linalg.norm(e)).astype(np.float32)
+                row += m
 
-        for k in range(min(2, len(batches))):
-            submit(k)
-        for k in range(len(batches)):
-            pool, jobs = groups.pop(k)
-            n_decoded, errs = collect_group(jobs)
-            decoded += n_decoded
-            n = sum(len(ids) for _, _, ids in batches[k][1])
-            norm = {} if self._norm[0] is None else {"mean": self._norm[0], "std": self._norm[1]}
-            if self._target_res is not None:
-                th, tw = self._target_res
-                small = self._ctx.resize_cubic_u8(pool, tw, th, slots=np.arange(n, dtype=np.int32), mode=self._cubic_mode)
-                emb, _, score = tower.embed_pool(self._ctx.rgb_pool(small), **norm)
-            else:
-                emb, _, score = tower.embed_pool(pool, slots=np.arange(n, dtype=np.int32), **norm)
-            score_h, emb_h = self._host_buffers(k % self.RING)
-            if score_h is not None:
-                score_h[:n].copy_(score, non_blocking=True)
-            if emb_h is not None:
-                emb_h[:n].copy_(emb, non_blocking=True)
-            ev = torch.cuda.Event()
-            ev.record(stream)
-            inflight[k] = (ev, jobs, errs, n)
-            if k >= 1:
-                finalize(k - 1)  # also frees the surface pool and host buffers batch k+2 is about to reuse
-            if k + 2 < len(batches):
-                submit(k + 2)
-        if batches:
-            finalize(len(batches) - 1)
-        self.last_call_stats = {"frames_decoded": decoded, "batches": len(batches), "nvdec_sessions": self._num_decoders,
-                                "numa_node": self._decode_pool.numa_node, "pinned_cpus": len(self._decode_pool.cpus)}  # fmt: skip
+        return write
 
     # ---- stage entry -----------------------------------------------------------------------------
     def process_data(self, tasks):
         self._timer.reinit(self, sum(task.get_major_size() for task in tasks))
         n_clips = sum(len(video.clips) for task in tasks for video in task.videos)
         with self._timer.time_process(num_samples=max(1, n_clips)):
-            by_size: dict[tuple[int, int], list] = {}
+            items = []
             for task in tasks:
                 for video in task.videos:
                     for clip in video.clips:
-                        plan = self._plan(clip, video)
-                        if plan is not None:
-                            data, ids, size = plan
-                            by_size.setdefault(size, []).append((clip, data, ids))
-            self._run_batches(self._make_batches(by_size))
+                        source = video if self._source == "video_span" else clip
+                        data = source.encoded_data.resolve() if source.encoded_data else None
+                        if data is None:
+                            logger.warning(f"Clip {clip.uuid} has no encoded_data (source={self._source}).")
+                            clip.errors["encoded_data"] = "empty"
+                            clip.aesthetic_score = -1.0
+                            continue
+                        items.append((clip, data))
+            # decode of batches k+1, k+2 (NVDEC + host parsing threads) overlaps preprocess + tower of batch k (SMs)
+            decoded, batches = run_decode_groups(items, self._plan, self._pools, lambda: self._decode_pool, self._compute,
+                                                 on_error=self._decode_failed, max_frames=self._max_batch, depth=self.RING,
+                                                 seek_keyframes=self._seek)  # fmt: skip
+            self.last_call_stats = {"frames_decoded": decoded, "batches": batches, "nvdec_sessions": self._num_decoders,
+                                    "numa_node": self._decode_pool.numa_node, "pinned_cpus": len(self._decode_pool.cpus)}  # fmt: skip
 
             for task in tasks:
                 for video in task.videos:

@@ -15,11 +15,10 @@ from __future__ import annotations
 import numpy as np
 
 from .. import sampling
-from .._lib import CurateB200Error
 from ..data_model import StageTimer
 from ..interfaces import CuratorStage, CuratorStageResource, ModelInterface
 from ..models.internvideo2_frames import InternVideo2FrameFormulator, select_frame_ids
-from ..runtime import DecoderPool, SurfacePools, check_colour, collect_group, even_size, get_context, mp4_index
+from ..runtime import DecoderPool, SurfacePools, check_colour, even_size, get_context, mp4_index, run_decode_groups
 from ..sampling import FrameExtractionPolicy, FrameExtractionSignature
 
 try:
@@ -67,67 +66,12 @@ def plan_clip(clip, data, target_fps: float, fn: int, verbose: bool = False):
     return even_size(idx["width"], idx["height"]), uniq.astype(np.int32), inverse.astype(np.int32)
 
 
-def run_decode_groups(items, plan, pools: SurfacePools, decoders, compute, *, on_short, on_error, group: int, depth: int = 2,
-                      seek_keyframes: bool = False, retire=None) -> tuple[int, int]:  # fmt: skip
-    """Decode the kept frames of clips [(clip, mp4 bytes)] into surface pools, group by group, and hand each group to `compute`.
-
-    plan(clip, data) gives plan_clip's result: None sends the clip to on_short(clip), CurateB200Error / ValueError to on_error(clip, e).
-    The planned clips are grouped per surface size, `group` clips at a time.  Group k is decoded by decoders() (a DecoderPool) into
-    pool k % depth of its size's ring while the groups before it compute.  compute(k, pool, clips, slots) gets the clips whose decode
-    succeeded (the others go to on_error) and their kept frames' surface indices, concatenated clip-major.  When compute only queues
-    GPU work, retire(k) must return once group k's work no longer reads its pool: a pool is decoded into again only after that.
-    -> (frames decoded, groups)."""
-    by_size: dict[tuple, list] = {}
-    for clip, data in items:
-        try:
-            planned = plan(clip, data)
-        except (CurateB200Error, ValueError) as e:
-            on_error(clip, e)
-            continue
-        if planned is None:
-            on_short(clip)
-            continue
-        by_size.setdefault(planned[0], []).append((clip, data, planned[1], planned[2]))
-    groups = [(size, clips[i : i + group]) for size, clips in by_size.items() for i in range(0, len(clips), group)]
-    ring_pos: dict[tuple, int] = {}
-    pending: dict[int, tuple] = {}
-
-    def submit(k):
-        size, clips = groups[k]
-        r = ring_pos.get(size, 0)
-        ring_pos[size] = (r + 1) % depth
-        pool = pools.get(size, sum(len(ids) for _, _, ids, _ in clips), r)
-        pending[k] = pool, decoders().submit_group(pool, size, [(data, ids) for _, data, ids, _ in clips], seek_keyframes)
-
-    decoded = 0
-    for k in range(min(depth - 1, len(groups))):
-        submit(k)
-    for k, (_, clips) in enumerate(groups):
-        pool, jobs = pending.pop(k)
-        n, errs = collect_group(jobs)
-        decoded += n
-        ok, slots = [], []
-        for (clip, _, _, inverse), (first, _), err in zip(clips, jobs, errs):
-            if err is not None:
-                on_error(clip, err)
-                continue
-            ok.append(clip)
-            slots.append(first + inverse)
-        if retire is not None and k >= 1:
-            retire(k - 1)
-        if k + depth - 1 < len(groups):
-            submit(k + depth - 1)  # the next groups decode while this one computes
-        if ok:
-            compute(k, pool, ok, np.concatenate(slots).astype(np.int32))
-    if retire is not None and groups:
-        retire(len(groups) - 1)
-    return decoded, len(groups)
-
-
 class InternVideo2FrameCreationStage(CuratorStage):
     """Stage for creating InternVideo2 input frames from video clips."""
 
-    GROUP = 32  # clips per decode group of the nvdec source (32 x 8 surfaces: 0.8 GB of 1080p NV12 per pool, two pools)
+    # clips per decode group of the nvdec source (32 x 8 surfaces: 0.8 GB of 1080p NV12 per pool, two pools).  A group's device tubes
+    # (32 x 8 x 3 x 224 x 224 fp32, 154 MB) are copied to the host only after the next group is queued: two groups' tubes at peak.
+    GROUP = 32
 
     def __init__(self, target_fps: float = 2.0, *, verbose: bool = False, log_stats: bool = False, source: str = "frames",
                  num_gpus_per_worker: float = 0.1, num_decoders: int = 8, stage_batch_size: int = 1, colour: str = "swscale",
@@ -185,12 +129,17 @@ class InternVideo2FrameCreationStage(CuratorStage):
             clip.intern_video_2_frames = np.empty(0, dtype=np.float32)
 
         def compute(k, pool, ok, slots):
-            tubes = self._model.formulate_pool(pool, slots).cpu().numpy()  # [len(ok) * fn, 3, s, s]
-            for i, clip in enumerate(ok):
-                clip.intern_video_2_frames = tubes[i * fn : (i + 1) * fn][None].copy()
+            tubes = self._model.formulate_pool(pool, slots)  # [len(ok) * fn, 3, s, s]
+
+            def write():
+                host = tubes.cpu().numpy()
+                for i, (clip, _) in enumerate(ok):
+                    clip.intern_video_2_frames = host[i * fn : (i + 1) * fn][None].copy()
+
+            return write
 
         run_decode_groups(items, lambda clip, data: plan_clip(clip, data, self._target_fps, fn, self._verbose), self._pools, self._decoders,
-                          compute, on_short=too_short, on_error=self._decode_failed, group=self.GROUP)  # fmt: skip
+                          compute, on_short=too_short, on_error=self._decode_failed, max_frames=self.GROUP * fn)  # fmt: skip
 
     @staticmethod
     def _decode_failed(clip, e) -> None:

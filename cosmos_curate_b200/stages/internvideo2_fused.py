@@ -7,8 +7,9 @@ the tower's patch rows (cb_iv2_embed_surfaces: one resize + normalise + patch-ro
 computes), and only the [n, 512] embeddings come back, through pinned host buffers.  The tube's frame count is the tower's own
 (model.get_target_num_frames(), read from pos_embed), so the formulator / tower frame-count pairing cannot go wrong.
 
-The frame plan (sampled ids from the MP4 index, the reference's re-extraction rule, the kept frames) and the decode-group loop are the
-frame-creation stage's own (plan_clip, run_decode_groups): the kept frames, the errors and the embeddings are the pair's.  Per clip:
+The frame plan (sampled ids from the MP4 index, the reference's re-extraction rule, the kept frames) is the frame-creation stage's own
+(plan_clip), and the decode-group loop is runtime.run_decode_groups, which that stage and NvdecClipAestheticStage run too: the kept
+frames, the errors and the embeddings are the pair's.  Per clip:
 
     no encoded_data                    -> errors {"encoded_data": "empty", "iv2_frames": "none"}, no embedding
     unreadable container / decode fail -> errors {"frame_extraction": "video_decode_failed", "iv2_frames": "none"}, no embedding
@@ -17,7 +18,7 @@ frame-creation stage's own (plan_clip, run_decode_groups): the kept frames, the 
 
 `clip.intern_video_2_frames` is never set.  Clips of all tasks of a call share decode groups and tower chunks; decode of the next
 groups overlaps the tower on the current one (a ring of RING surface pools per resolution, one pinned host buffer per ring slot, each
-reused only after its event has fired).
+reused only after the loop has waited on the event of the group that last used it).
 """
 
 from __future__ import annotations
@@ -28,9 +29,9 @@ import torch
 from ..data_model import StageTimer
 from ..interfaces import CuratorStage, CuratorStageResource, ModelInterface
 from ..models.internvideo2 import InternVideo2MultiModality
-from ..runtime import IMAGENET_MEAN, IMAGENET_STD, DecoderPool, SurfacePools, check_colour, get_context, nvdec_available
+from ..runtime import IMAGENET_MEAN, IMAGENET_STD, DecoderPool, SurfacePools, check_colour, get_context, nvdec_available, run_decode_groups
 from .internvideo2_embedding import TextMatch
-from .internvideo2_frames import InternVideo2FrameCreationStage, plan_clip, run_decode_groups
+from .internvideo2_frames import InternVideo2FrameCreationStage, plan_clip
 
 try:
     from loguru import logger
@@ -108,10 +109,9 @@ class NvdecInternVideo2EmbeddingStage(CuratorStage):
         clip.errors["iv2_frames"] = "empty"
 
     def _embed(self, items) -> None:
-        """items: [(clip, mp4 bytes)] -> embeddings on the clips.  Group k's tower work and D2H copy are queued, then group k - 1's
-        results are written once its event has fired; its surface pool and host buffer are reused only after that."""
-        tower, stream, fn, bs = self._model.tower, torch.cuda.current_stream(), self._frames, self._batch_size
-        inflight: dict[int, tuple] = {}
+        """items: [(clip, mp4 bytes)] -> embeddings on the clips.  Group k's tower work and D2H copy into the pinned buffer of its ring
+        slot are queued; the buffer is read once group k's event has fired."""
+        tower, fn, bs = self._model.tower, self._frames, self._batch_size
 
         def compute(k, pool, ok, slots):
             host = self._host_buffer(k % self.RING, len(ok), tower.embed_dim)
@@ -119,21 +119,16 @@ class NvdecInternVideo2EmbeddingStage(CuratorStage):
                 m = min(bs, len(ok) - i)
                 emb = tower.embed_pool(pool, slots[i * fn : (i + m) * fn], mean=IMAGENET_MEAN, std=IMAGENET_STD)
                 host[i : i + m].copy_(emb, non_blocking=True)
-            ev = torch.cuda.Event()
-            ev.record(stream)
-            inflight[k] = (ev, ok, host)
 
-        def retire(k):
-            if k not in inflight:  # no clip of the group decoded
-                return
-            ev, ok, host = inflight.pop(k)
-            ev.synchronize()
-            for i, clip in enumerate(ok):
-                clip.intern_video_2_embedding = host[i : i + 1].numpy().copy()
+            def write():
+                for i, (clip, _) in enumerate(ok):
+                    clip.intern_video_2_embedding = host[i : i + 1].numpy().copy()
+
+            return write
 
         decoded, groups = run_decode_groups(items, lambda clip, data: plan_clip(clip, data, self._target_fps, fn, self._verbose), self._pools,
                                             lambda: self._decode_pool, compute, on_short=self._too_short, on_error=self._decode_failed,
-                                            group=self.GROUP, depth=self.RING, seek_keyframes=self._seek, retire=retire)  # fmt: skip
+                                            max_frames=self.GROUP * fn, depth=self.RING, seek_keyframes=self._seek)  # fmt: skip
         self.last_call_stats = {"frames_decoded": decoded, "groups": groups, "nvdec_sessions": self._num_decoders,
                                 "host_decode": not nvdec_available(self._ctx)}  # fmt: skip
 

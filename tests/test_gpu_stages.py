@@ -413,27 +413,37 @@ def test_fused_stage_keyframe_seek_gives_identical_results(ctx):
 
 def test_fused_stage_mixed_resolutions_in_one_call(ctx):
     """BASELINE.json configs[4] mixes 720p / 1080p / 4K clips in one stream: clips of different sizes inside ONE process_data call go
-    through per-resolution surface-pool rings and batches; every clip gets the score it gets when processed alone."""
+    through per-resolution surface-pool rings and batches; every clip gets the score it gets when processed alone, also the clips
+    that share a batch with a clip whose decode fails."""
+    import struct
+
     from cosmos_curate_b200.data_model import Clip
     from cosmos_curate_b200.stages import NvdecClipAestheticStage
     from tools import synth_h264
 
+    # 640x368 like sources[0], a valid index, every sample's NAL length past the sample: demuxes, fails to decode
+    undecodable = synth_h264.mux_mp4([struct.pack(">I", 1 << 20) + bytes(16)] * 60, [i % 30 == 0 for i in range(60)], synth_h264.sps(640, 368, 30),
+                                     synth_h264.pps(), 640, 368, 30)  # fmt: skip
     sources = [synth_h264.make_coded_clip(640, 368, 30, 2.0, seed=31, bitrate=1.0e6), synth_h264.make_coded_clip(1280, 720, 30, 2.0, seed=32, bitrate=2.0e6),
-               (GOLDEN / "sintel_clip_10s.mp4").read_bytes(), synth_h264.make_coded_clip(1920, 1080, 30, 2.0, seed=33, bitrate=4.0e6)]
+               (GOLDEN / "sintel_clip_10s.mp4").read_bytes(), synth_h264.make_coded_clip(1920, 1080, 30, 2.0, seed=33, bitrate=4.0e6), undecodable]
     model, cfg, w, sd = _model()
     stage = NvdecClipAestheticStage(score_threshold=-100.0, reduction="mean", write_embedding=True, max_batch=16, num_decoders=4, model=model)
     stage.stage_setup()
     alone = []
-    for s in sources:
+    for s in sources[:4]:
         t = _clip_task(s)
         stage.process_data([t])
         alone.append((t.video.clips[0].aesthetic_score, t.video.clips[0].openai_embedding))
-    order = [0, 1, 2, 3, 1, 0, 3, 2, 2, 1]  # interleaved sizes, more frames than one batch holds (max_batch = 16)
+    # interleaved sizes, more frames than one batch holds (max_batch = 16); the undecodable clip (4) shares a batch with two of 0
+    order = [0, 1, 4, 2, 3, 1, 0, 3, 2, 2, 1]
     task = _clip_task(sources[0], n_clips=0)
     task.video.clips = [Clip(uuid=uuid.uuid4(), source_video="v.mp4", span=(0.0, 2.0), encoded_data=sources[k]) for k in order]
     stage.process_data([task])
     assert len(task.video.clips) == len(order)
     for clip, k in zip(task.video.clips, order):
+        if k == 4:
+            assert clip.errors == {"frame_extraction": "video_decode_failed"} and clip.aesthetic_score == -1.0 and clip.openai_embedding is None
+            continue
         assert clip.aesthetic_score == alone[k][0] and np.array_equal(clip.openai_embedding, alone[k][1]), k
     assert stage.last_call_stats["batches"] >= 4
     stage.destroy()
