@@ -75,6 +75,15 @@ class Iv2TextCfg(C.Structure):
     ]  # fmt: skip
 
 
+class TransnetConvArgs(C.Structure):
+    """cb_transnet_conv_args: one launch of the shot network's gather-GEMM (device pointers as ints)."""
+
+    _fields_ = [("in_", C.c_void_p), ("w", C.c_void_p), ("out", C.c_void_p), ("scale", C.c_void_p), ("shift", C.c_void_p)] + [
+        (name, C.c_int) for name in ("M", "N", "cin", "in_ld", "in_coff", "w_ld", "out_ld", "out_coff", "T", "H", "W", "mode", "dil", "relu",
+                                     "z_in_coff", "z_out_coff", "z_dil_shift")
+    ] + [("z_w", C.c_longlong)]  # fmt: skip
+
+
 class Mp4Info(C.Structure):
     _fields_ = [
         ("codec", C.c_int), ("width", C.c_int), ("height", C.c_int), ("timescale", C.c_uint32),
@@ -134,6 +143,13 @@ SIGNATURES = {
     "cb_transnet_finalize": (_i, [_vp, _i]),
     "cb_transnet_forward": (_i, [_vp, _vp, _i, _i, _vp, _vp]),
     "cb_transnet_predict": (_i, [_vp, _vp, _i, _vp, _vp]),
+    "cb_transnet_conv": (_i, [_vp, C.POINTER(TransnetConvArgs), _i, _vp]),
+    "cb_transnet_window_gather": (_i, [_vp, _vp, _vp, _vp, _i, _i, _vp, _vp, _vp]),
+    "cb_transnet_shortcut_pool": (_i, [_vp, _vp, _vp, _vp, _i, _i, _i, _i, C.c_longlong, _vp]),
+    "cb_transnet_spatial_mean": (_i, [_vp, _vp, C.c_longlong, _i, _i, _i, _vp, _i, _i, _vp]),
+    "cb_transnet_l2_normalize_rows": (_i, [_vp, _vp, _i, _i, _vp]),
+    "cb_transnet_window_similarity_fc": (_i, [_vp, _vp, _i, _i, _i, _vp, _vp, _vp, _i, _i, _vp]),
+    "cb_transnet_head": (_i, [_vp, _vp, _vp, _f, _i, _i, _vp, _i, _i, _i, _vp]),
     "cb_rowdot_argmax": (_i, [_vp, _vp, _i, _vp, _i, _i, _vp, _i, _f, _vp, _vp, _vp]),
     "cb_rows_l2_normalize": (_i, [_vp, _vp, _i, _i, _vp, _vp]),
     "cb_cluster_sums": (_i, [_vp, _vp, _vp, _vp, _i, _i, _vp, _vp]),

@@ -385,6 +385,109 @@ static int conv_dispatch(cb_ctx* ctx, const ConvGemmArgs& a, int zdim, cudaStrea
   return fail(ctx, CB_ERR_UNSUPPORTED, "transnet: no conv kernel for cin=%d N=%d", a.cin, a.N);
 }
 
+static bool aligned16(const void* p) { return ((uintptr_t)p & 15) == 0; }  // NULL counts as aligned
+
+// One launch of conv_gemm_kernel over zdim branches.  Everything the float4 loads and stores need is checked here: the base
+// pointers, and every row stride and column offset a multiple of 4 floats.  Modes 1 and 2 gather taps inside a frame (mode 1) or
+// a window (mode 2), so M must hold whole frames, and for mode 2 whole windows: a tap of the last window would otherwise read rows
+// past M.
+static int conv(cb_ctx* ctx, const ConvGemmArgs& a, int zdim, cudaStream_t st) {
+  if (!a.in || !a.w || !a.out) return fail(ctx, CB_ERR_ARG, "transnet conv: null operand");
+  if (a.mode < 0 || a.mode > 2) return fail(ctx, CB_ERR_ARG, "transnet conv: mode=%d (0 rows, 1 spatial taps, 2 temporal taps)", a.mode);
+  if (zdim < 1 || zdim > 65535) return fail(ctx, CB_ERR_ARG, "transnet conv: z=%d (1..65535)", zdim);
+  if (a.M < 0 || a.N <= 0 || a.cin <= 0 || a.T <= 0 || a.H <= 0 || a.W <= 0 || a.dil < 0 || a.z_dil_shift < 0)
+    return fail(ctx, CB_ERR_ARG, "transnet conv: M=%d N=%d cin=%d T=%d H=%d W=%d dil=%d", a.M, a.N, a.cin, a.T, a.H, a.W, a.dil);
+  if (!aligned16(a.in) || !aligned16(a.w) || !aligned16(a.out) || ((uintptr_t)a.scale & 3) || ((uintptr_t)a.shift & 3))
+    return fail(ctx, CB_ERR_ARG, "transnet conv: in, w and out must be 16-byte aligned, scale and shift 4-byte");
+  if ((a.in_ld | a.in_coff | a.out_ld | a.out_coff | a.w_ld | a.z_in_coff | a.z_out_coff | (int)(a.z_w & 3)) & 3 || a.in_ld < 0 || a.in_coff < 0 ||
+      a.out_ld < 0 || a.out_coff < 0 || a.w_ld < 0 || a.z_in_coff < 0 || a.z_out_coff < 0 || a.z_w < 0)
+    return fail(ctx, CB_ERR_ARG, "transnet conv: in_ld=%d in_coff=%d out_ld=%d out_coff=%d w_ld=%d z_in_coff=%d z_out_coff=%d z_w=%lld must be multiples of 4",
+                a.in_ld, a.in_coff, a.out_ld, a.out_coff, a.w_ld, a.z_in_coff, a.z_out_coff, a.z_w);
+  const long long frame = (long long)a.H * a.W, rows_per_unit = a.mode == 2 ? frame * a.T : (a.mode == 1 ? frame : 1);
+  if (a.M % rows_per_unit) return fail(ctx, CB_ERR_ARG, "transnet conv: M=%d is not a whole number of %s of %lld rows", a.M, a.mode == 2 ? "windows" : "frames", rows_per_unit);
+  if (a.M == 0) return CB_OK;
+  return conv_dispatch(ctx, a, zdim, st);
+}
+
+static int window_gather(cb_ctx* ctx, const uint8_t* frames, const int* first, const int* pad, int B, int T, float* x0, float* hist, cudaStream_t st) {
+  if (!frames || !first || !pad || !x0 || !hist) return fail(ctx, CB_ERR_ARG, "transnet window_gather: null operand");
+  if (B < 0 || T < 0 || (long long)B * T > INT32_MAX) return fail(ctx, CB_ERR_ARG, "transnet window_gather: B=%d T=%d", B, T);
+  if (!aligned16(x0) || ((uintptr_t)first & 3) || ((uintptr_t)pad & 3) || ((uintptr_t)hist & 3))
+    return fail(ctx, CB_ERR_ARG, "transnet window_gather: x0 must be 16-byte aligned, first, pad and hist 4-byte");
+  if (B == 0 || T == 0) return CB_OK;
+  mark_launch(ctx, CB_PROF_CONV, st);
+  window_gather_kernel<<<B * T, 256, 0, st>>>(frames, first, pad, T, x0, hist);
+  CB_CUDA(ctx, cudaGetLastError());
+  return CB_OK;
+}
+
+static int shortcut_pool(cb_ctx* ctx, const float* x2, const float* x1, float* out, int frames, int H, int W, int C, long long out_frame_stride, cudaStream_t st) {
+  if (!x2 || !x1 || !out) return fail(ctx, CB_ERR_ARG, "transnet shortcut_pool: null operand");
+  if (frames < 0 || H < 0 || W < 0 || C < 0 || out_frame_stride < 0)
+    return fail(ctx, CB_ERR_ARG, "transnet shortcut_pool: frames=%d H=%d W=%d C=%d out_frame_stride=%lld", frames, H, W, C, out_frame_stride);
+  if (!aligned16(x2) || !aligned16(x1) || !aligned16(out) || C % 4 || out_frame_stride % 4)
+    return fail(ctx, CB_ERR_ARG, "transnet shortcut_pool: x2, x1, out must be 16-byte aligned, C=%d and out_frame_stride=%lld multiples of 4", C, out_frame_stride);
+  const long long total = (long long)frames * (H / 2) * (W / 2) * (C / 4);
+  if (total == 0) return CB_OK;
+  const int blocks = (int)std::min<long long>((total + 255) / 256, 148LL * 16);
+  mark_launch(ctx, CB_PROF_CONV, st);
+  shortcut_pool_kernel<<<blocks, 256, 0, st>>>(x2, x1, out, frames, H, W, C, out_frame_stride);
+  CB_CUDA(ctx, cudaGetLastError());
+  return CB_OK;
+}
+
+static int spatial_mean(cb_ctx* ctx, const float* x, long long frame_stride, int frames, int npos, int C, float* feats, int feats_ld, int coff, cudaStream_t st) {
+  if (!x || !feats) return fail(ctx, CB_ERR_ARG, "transnet spatial_mean: null operand");
+  if (frames < 0 || npos <= 0 || C < 0 || frame_stride < 0 || feats_ld < 0 || coff < 0)
+    return fail(ctx, CB_ERR_ARG, "transnet spatial_mean: frames=%d npos=%d C=%d frame_stride=%lld feats_ld=%d coff=%d", frames, npos, C, frame_stride, feats_ld, coff);
+  if (((uintptr_t)x & 3) || ((uintptr_t)feats & 3)) return fail(ctx, CB_ERR_ARG, "transnet spatial_mean: x and feats must be 4-byte aligned");
+  if (frames == 0 || C == 0) return CB_OK;
+  mark_launch(ctx, CB_PROF_CONV, st);
+  spatial_mean_kernel<<<frames, 128, 0, st>>>(x, frame_stride, npos, C, feats, feats_ld, coff);
+  CB_CUDA(ctx, cudaGetLastError());
+  return CB_OK;
+}
+
+static int l2_normalize_rows(cb_ctx* ctx, float* x, int rows, int D, cudaStream_t st) {
+  if (!x) return fail(ctx, CB_ERR_ARG, "transnet l2_normalize_rows: null operand");
+  if (rows < 0 || D <= 0) return fail(ctx, CB_ERR_ARG, "transnet l2_normalize_rows: rows=%d D=%d", rows, D);
+  if ((uintptr_t)x & 3) return fail(ctx, CB_ERR_ARG, "transnet l2_normalize_rows: x must be 4-byte aligned");
+  if (rows == 0) return CB_OK;
+  mark_launch(ctx, CB_PROF_CONV, st);
+  l2_normalize_rows_kernel<<<rows, 128, 0, st>>>(x, D);
+  CB_CUDA(ctx, cudaGetLastError());
+  return CB_OK;
+}
+
+// rows = whole windows of T frames: every neighbour a row reads is a row of its own window.
+static int window_similarity_fc(cb_ctx* ctx, const float* x, int rows, int D, int T, const float* wt, const float* bias, float* out, int out_ld, int out_coff,
+                                cudaStream_t st) {
+  if (!x || !wt || !bias || !out) return fail(ctx, CB_ERR_ARG, "transnet window_similarity_fc: null operand");
+  if (rows < 0 || D <= 0 || T <= 0 || rows % T || out_ld < 0 || out_coff < 0)
+    return fail(ctx, CB_ERR_ARG, "transnet window_similarity_fc: rows=%d D=%d T=%d out_ld=%d out_coff=%d (rows whole windows of T)", rows, D, T, out_ld, out_coff);
+  if (((uintptr_t)x & 3) || ((uintptr_t)wt & 3) || ((uintptr_t)bias & 3) || ((uintptr_t)out & 3))
+    return fail(ctx, CB_ERR_ARG, "transnet window_similarity_fc: operands must be 4-byte aligned");
+  const size_t smem = ((size_t)D + kLookup) * sizeof(float);
+  if (smem > 48 * 1024) return fail(ctx, CB_ERR_UNSUPPORTED, "transnet window_similarity_fc: D=%d: %zu bytes of shared memory exceed 48 KB", D, smem);
+  if (rows == 0) return CB_OK;
+  mark_launch(ctx, CB_PROF_CONV, st);
+  window_similarity_fc_kernel<<<rows, 128, smem, st>>>(x, D, T, wt, bias, out, out_ld, out_coff);
+  CB_CUDA(ctx, cudaGetLastError());
+  return CB_OK;
+}
+
+static int head(cb_ctx* ctx, const float* h, const float* w, float bias, int rows, int T, float* prob, int stitch, int w0, int n_total, cudaStream_t st) {
+  if (!h || !w || !prob) return fail(ctx, CB_ERR_ARG, "transnet head: null operand");
+  if (rows < 0 || T <= 0 || (stitch != 0 && stitch != 1) || w0 < 0 || n_total < 0)
+    return fail(ctx, CB_ERR_ARG, "transnet head: rows=%d T=%d stitch=%d w0=%d n_total=%d", rows, T, stitch, w0, n_total);
+  if (((uintptr_t)h & 3) || ((uintptr_t)w & 3) || ((uintptr_t)prob & 3)) return fail(ctx, CB_ERR_ARG, "transnet head: operands must be 4-byte aligned");
+  if (rows == 0) return CB_OK;
+  mark_launch(ctx, CB_PROF_CONV, st);
+  head_kernel<<<(rows + 3) / 4, 128, 0, st>>>(h, w, bias, rows, T, prob, stitch, w0, n_total);
+  CB_CUDA(ctx, cudaGetLastError());
+  return CB_OK;
+}
+
 // B windows of T frames each; window b = video frames first[b] + max(t - pad[b], 0).  prob: see head_kernel.
 static int run_windows(cb_transnet* tn, const uint8_t* frames, const int* h_first, const int* h_pad, int B, int T, float* prob, int stitch, int w0, int n_total,
                        cudaStream_t st) {
@@ -392,11 +495,9 @@ static int run_windows(cb_transnet* tn, const uint8_t* frames, const int* h_firs
   CB_CUDA(ctx, cudaMemcpyAsync(tn->d_first, h_first, B * sizeof(int), cudaMemcpyHostToDevice, st));
   CB_CUDA(ctx, cudaMemcpyAsync(tn->d_pad, h_pad, B * sizeof(int), cudaMemcpyHostToDevice, st));
   const int frames_n = B * T;
-  mark_launch(ctx, CB_PROF_CONV, st);
-  window_gather_kernel<<<frames_n, 256, 0, st>>>(frames, tn->d_first, tn->d_pad, T, tn->x0, tn->hist);
-  CB_CUDA(ctx, cudaGetLastError());
-
   int rc;
+  if ((rc = window_gather(ctx, frames, tn->d_first, tn->d_pad, B, T, tn->x0, tn->hist, st))) return rc;
+
   int H = kFrameH, W = kFrameW;
   const float* x = tn->x0;
   int x_ld = 4;
@@ -410,29 +511,21 @@ static int run_windows(cb_transnet* tn, const uint8_t* frames, const int* h_firs
       a.in = x, a.w = k.w1, a.out = tn->mid, a.scale = nullptr, a.shift = nullptr;
       a.M = M, a.N = 8 * f, a.cin = k.cin_pad, a.in_ld = x_ld, a.in_coff = 0, a.w_ld = 8 * f, a.out_ld = 8 * f, a.out_coff = 0;
       a.T = T, a.H = H, a.W = W, a.mode = 1, a.dil = 1, a.relu = 0;
-      if ((rc = conv_dispatch(ctx, a, 1, st))) return rc;
+      if ((rc = conv(ctx, a, 1, st))) return rc;
       ConvGemmArgs t{};
       t.in = tn->mid, t.w = k.w2, t.out = outs[b], t.scale = k.scale, t.shift = k.shift;
       t.M = M, t.N = f, t.cin = 2 * f, t.in_ld = 8 * f, t.in_coff = 0, t.w_ld = f, t.out_ld = C, t.out_coff = 0;
       t.T = T, t.H = H, t.W = W, t.mode = 2, t.relu = k.relu ? 1 : 0;
       t.z_in_coff = 2 * f, t.z_out_coff = f, t.z_w = (long long)3 * 2 * f * f;
       t.dil = 1, t.z_dil_shift = 1;  // branch z: dilation 1 << z, its own channel slices and weights
-      if ((rc = conv_dispatch(ctx, t, kBranches, st))) return rc;
+      if ((rc = conv(ctx, t, kBranches, st))) return rc;
       x = outs[b], x_ld = C;
     }
     const int Hp = H / 2, Wp = W / 2;
     float* pooled = s == 0 ? tn->p0 : (s == 1 ? tn->p1 : tn->concat + kTrunkOff);
     const long long fstride = s == 2 ? kFcIn : (long long)Hp * Wp * C;
-    {
-      const long long total = (long long)frames_n * Hp * Wp * (C / 4);
-      const int blocks = (int)std::min<long long>((total + 255) / 256, 148LL * 16);
-      mark_launch(ctx, CB_PROF_CONV, st);
-      shortcut_pool_kernel<<<blocks, 256, 0, st>>>(tn->b2, tn->b1, pooled, frames_n, H, W, C, fstride);
-      CB_CUDA(ctx, cudaGetLastError());
-      mark_launch(ctx, CB_PROF_CONV, st);
-      spatial_mean_kernel<<<frames_n, 128, 0, st>>>(pooled, fstride, Hp * Wp, C, tn->feats, 448, feat_off);
-      CB_CUDA(ctx, cudaGetLastError());
-    }
+    if ((rc = shortcut_pool(ctx, tn->b2, tn->b1, pooled, frames_n, H, W, C, fstride, st))) return rc;
+    if ((rc = spatial_mean(ctx, pooled, fstride, frames_n, Hp * Wp, C, tn->feats, 448, feat_off, st))) return rc;
     feat_off += C;
     x = pooled, x_ld = C, H = Hp, W = Wp;
   }
@@ -442,28 +535,18 @@ static int run_windows(cb_transnet* tn, const uint8_t* frames, const int* h_firs
     a.in = tn->feats, a.w = tn->proj_wt, a.out = tn->proj, a.shift = tn->proj_b;
     a.M = frames_n, a.N = kSimDim, a.cin = 448, a.in_ld = 448, a.w_ld = kSimDim, a.out_ld = kSimDim;
     a.T = T, a.H = 1, a.W = 1, a.mode = 0;
-    if ((rc = conv_dispatch(ctx, a, 1, st))) return rc;
-    mark_launch(ctx, CB_PROF_CONV, st);
-    l2_normalize_rows_kernel<<<frames_n, 128, 0, st>>>(tn->proj, kSimDim);
-    CB_CUDA(ctx, cudaGetLastError());
-    mark_launch(ctx, CB_PROF_CONV, st);
-    window_similarity_fc_kernel<<<frames_n, 128, (kSimDim + kLookup) * sizeof(float), st>>>(tn->proj, kSimDim, T, tn->sim_fc_wt, tn->sim_fc_b, tn->concat, kFcIn,
-                                                                                           kSimDim);
-    CB_CUDA(ctx, cudaGetLastError());
-    mark_launch(ctx, CB_PROF_CONV, st);
-    window_similarity_fc_kernel<<<frames_n, 128, (kHistBins + kLookup) * sizeof(float), st>>>(tn->hist, kHistBins, T, tn->hist_fc_wt, tn->hist_fc_b, tn->concat,
-                                                                                             kFcIn, 0);
-    CB_CUDA(ctx, cudaGetLastError());
+    if ((rc = conv(ctx, a, 1, st))) return rc;
+    if ((rc = l2_normalize_rows(ctx, tn->proj, frames_n, kSimDim, st))) return rc;
+    if ((rc = window_similarity_fc(ctx, tn->proj, frames_n, kSimDim, T, tn->sim_fc_wt, tn->sim_fc_b, tn->concat, kFcIn, kSimDim, st))) return rc;
+    if ((rc = window_similarity_fc(ctx, tn->hist, frames_n, kHistBins, T, tn->hist_fc_wt, tn->hist_fc_b, tn->concat, kFcIn, 0, st))) return rc;
   }
   {
     ConvGemmArgs a{};
     a.in = tn->concat, a.w = tn->fc1_wt, a.out = tn->fc1, a.shift = tn->fc1_b;
     a.M = frames_n, a.N = kFcOut, a.cin = kFcIn, a.in_ld = kFcIn, a.w_ld = kFcOut, a.out_ld = kFcOut;
     a.T = T, a.H = 1, a.W = 1, a.mode = 0, a.relu = 1;
-    if ((rc = conv_dispatch(ctx, a, 1, st))) return rc;
-    mark_launch(ctx, CB_PROF_CONV, st);
-    head_kernel<<<(frames_n + 3) / 4, 128, 0, st>>>(tn->fc1, tn->cls_w, tn->cls_b, frames_n, T, prob, stitch, w0, n_total);
-    CB_CUDA(ctx, cudaGetLastError());
+    if ((rc = conv(ctx, a, 1, st))) return rc;
+    if ((rc = head(ctx, tn->fc1, tn->cls_w, tn->cls_b, frames_n, T, prob, stitch, w0, n_total, st))) return rc;
   }
   return CB_OK;
 }
@@ -624,6 +707,48 @@ int cb_transnet_predict(cb_transnet* tn, const uint8_t* frames, int n_frames, fl
     w += B;
   }
   return CB_OK;
+}
+
+int cb_transnet_conv(cb_ctx* ctx, const cb_transnet_conv_args* a, int z, void* stream) {
+  if (!ctx) return CB_ERR_ARG;
+  if (!a) return cb::fail(ctx, CB_ERR_ARG, "transnet conv: null argument");
+  cb::ConvGemmArgs g{};
+  g.in = a->in, g.w = a->w, g.out = a->out, g.scale = a->scale, g.shift = a->shift;
+  g.M = a->M, g.N = a->N, g.cin = a->cin, g.in_ld = a->in_ld, g.in_coff = a->in_coff, g.w_ld = a->w_ld, g.out_ld = a->out_ld, g.out_coff = a->out_coff;
+  g.T = a->T, g.H = a->H, g.W = a->W, g.mode = a->mode, g.dil = a->dil, g.relu = a->relu;
+  g.z_in_coff = a->z_in_coff, g.z_out_coff = a->z_out_coff, g.z_dil_shift = a->z_dil_shift, g.z_w = a->z_w;
+  return cb::conv(ctx, g, z, (cudaStream_t)stream);
+}
+
+int cb_transnet_window_gather(cb_ctx* ctx, const uint8_t* frames, const int32_t* first, const int32_t* pad, int B, int T, float* x0, float* hist, void* stream) {
+  if (!ctx) return CB_ERR_ARG;
+  return cb::window_gather(ctx, frames, first, pad, B, T, x0, hist, (cudaStream_t)stream);
+}
+
+int cb_transnet_shortcut_pool(cb_ctx* ctx, const float* x2, const float* x1, float* out, int frames, int H, int W, int C, long long out_frame_stride, void* stream) {
+  if (!ctx) return CB_ERR_ARG;
+  return cb::shortcut_pool(ctx, x2, x1, out, frames, H, W, C, out_frame_stride, (cudaStream_t)stream);
+}
+
+int cb_transnet_spatial_mean(cb_ctx* ctx, const float* x, long long frame_stride, int frames, int npos, int C, float* feats, int feats_ld, int coff, void* stream) {
+  if (!ctx) return CB_ERR_ARG;
+  return cb::spatial_mean(ctx, x, frame_stride, frames, npos, C, feats, feats_ld, coff, (cudaStream_t)stream);
+}
+
+int cb_transnet_l2_normalize_rows(cb_ctx* ctx, float* x, int rows, int D, void* stream) {
+  if (!ctx) return CB_ERR_ARG;
+  return cb::l2_normalize_rows(ctx, x, rows, D, (cudaStream_t)stream);
+}
+
+int cb_transnet_window_similarity_fc(cb_ctx* ctx, const float* x, int rows, int D, int T, const float* wt, const float* bias, float* out, int out_ld, int out_coff,
+                                     void* stream) {
+  if (!ctx) return CB_ERR_ARG;
+  return cb::window_similarity_fc(ctx, x, rows, D, T, wt, bias, out, out_ld, out_coff, (cudaStream_t)stream);
+}
+
+int cb_transnet_head(cb_ctx* ctx, const float* h, const float* w, float bias, int rows, int T, float* prob, int stitch, int w0, int n_total, void* stream) {
+  if (!ctx) return CB_ERR_ARG;
+  return cb::head(ctx, h, w, bias, rows, T, prob, stitch, w0, n_total, (cudaStream_t)stream);
 }
 
 }  // extern "C"

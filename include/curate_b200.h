@@ -303,6 +303,50 @@ int cb_transnet_forward(cb_transnet* tn, const uint8_t* windows, int n_windows, 
  * the tail windows left short exactly as _get_batches leaves them).  Thresholding (prob > threshold) is the caller's. */
 int cb_transnet_predict(cb_transnet* tn, const uint8_t* frames, int n_frames, float* prob_out, void* stream);
 
+/* The network's kernels one launch at a time, each with the checks cb_transnet_forward runs before it launches them.  Every
+ * pointer is device memory; a null operand or a misaligned pointer, stride or offset returns CB_ERR_ARG, zero rows is a no-op.
+ *
+ * The convolutions and Linear layers: out[m][out_coff + z * z_out_coff + n] = epi(sum_k A[m][k] * Wt[k][n]) for each branch z < `z`,
+ * k = (tap, c) tap-major, Wt = w + z * z_w with row stride w_ld, A[m][(tap, c)] = in[src][in_coff + z * z_in_coff + c] with row stride
+ * in_ld.  Row m is the position (frame m / (H W), row, col), frame t = (m / (H W)) % T of its window.
+ *   mode 0: one tap, src = m.
+ *   mode 1: 3 x 3 spatial taps (dh, dw) in row-major order, src = m + dh W + dw, zero outside the frame; M whole frames.
+ *   mode 2: 3 temporal taps dt = (tap - 1) * (dil << (z_dil_shift ? z : 0)), src = m + dt H W, zero outside the WINDOW; M whole
+ *           windows.
+ * epi: fmaf(acc, scale[c], shift[c]) with scale, else acc + shift[c] (shift NULL: + 0), c = out_coff + z * z_out_coff + n; then
+ * fmaxf(., 0) with relu.  in, w, out 16-byte aligned; in_ld, in_coff, out_ld, out_coff, w_ld, z_in_coff, z_out_coff and z_w multiples of
+ * 4.  N must be a multiple of 4, and with cin % 16 != 0 also cin % 4 == 0 and N >= 128 (CB_ERR_UNSUPPORTED). */
+typedef struct cb_transnet_conv_args {
+  const float* in;
+  const float* w;
+  float* out;
+  const float* scale; /* nullable */
+  const float* shift; /* nullable */
+  int M, N, cin, in_ld, in_coff, w_ld, out_ld, out_coff;
+  int T, H, W, mode, dil, relu;
+  int z_in_coff, z_out_coff, z_dil_shift;
+  long long z_w;
+} cb_transnet_conv_args;
+int cb_transnet_conv(cb_ctx* ctx, const cb_transnet_conv_args* args, int z, void* stream);
+/* frames uint8 [n][27][48][3]; window b < B, frame t < T is video frame first[b] + max(t - pad[b], 0) (first, pad device int32 [B]).
+ * x0 fp32 [B T][27][48][4] = rgb / 255 and 0, hist fp32 [B T][512] = the L2-normalised 3-bit-per-channel RGB histogram. */
+int cb_transnet_window_gather(cb_ctx* ctx, const uint8_t* frames, const int32_t* first, const int32_t* pad, int B, int T, float* x0, float* hist, void* stream);
+/* out[f][ho][wo][c] (frame stride out_frame_stride floats) = 0.25 * sum over the 2 x 2 block of (relu(x2) + x1), x2 and x1 fp32
+ * [frames][H][W][C]; H and W rounded down to even.  C and out_frame_stride multiples of 4. */
+int cb_transnet_shortcut_pool(cb_ctx* ctx, const float* x2, const float* x1, float* out, int frames, int H, int W, int C, long long out_frame_stride, void* stream);
+/* feats[f][coff + c] (row stride feats_ld) = the mean over npos >= 1 positions of x[f][p][c] (frame stride frame_stride floats). */
+int cb_transnet_spatial_mean(cb_ctx* ctx, const float* x, long long frame_stride, int frames, int npos, int C, float* feats, int feats_ld, int coff, void* stream);
+/* x fp32 [rows][D] in place: each row divided by max(|row|, 1e-12). */
+int cb_transnet_l2_normalize_rows(cb_ctx* ctx, float* x, int rows, int D, void* stream);
+/* rows = whole windows of T frames of x fp32 [rows][D]: out[r][out_coff + o] (row stride out_ld, o < 128) = relu(bias[o] + sum_j
+ * sim[r][j] wt[j][o]), sim[r][j] = x[r] . x[r + j - 50] for the 101 neighbours in the same window, 0 outside it.  wt [101][128].
+ * (D + 101) * 4 bytes must fit 48 KB of shared memory (CB_ERR_UNSUPPORTED). */
+int cb_transnet_window_similarity_fc(cb_ctx* ctx, const float* x, int rows, int D, int T, const float* wt, const float* bias, float* out, int out_ld, int out_coff,
+                                     void* stream);
+/* p = sigmoid(h[r] . w + bias), h fp32 [rows][1024].  stitch 0: prob[r] = p.  stitch 1: rows are windows w0, w0 + 1, ... of T
+ * frames; frames 25..74 of window w land at prob[50 w + t - 25] when that is < n_total, no other element is written. */
+int cb_transnet_head(cb_ctx* ctx, const float* h, const float* w, float bias, int rows, int T, float* prob, int stitch, int w0, int n_total, void* stream);
+
 /* ---- semantic dedup on the gathered embeddings (fp32) ------------------------------------------------ */
 #define CB_ROWDOT_UPPER 1 /* a == b: only candidates i < j count (strict upper triangle) */
 #define CB_ROWDOT_CLIP 2  /* clamp scores to [-1, 1] before comparing */
