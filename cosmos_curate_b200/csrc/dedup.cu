@@ -8,7 +8,9 @@
 //   KMeansMG centroid update                                                     -> cluster_sum_kernel (deterministic, no atomics)
 // fp32 on the SIMT pipes on purpose: the pruning decision is `max cosine <= 1 - eps` on near-duplicate pairs (cosine ~ 0.99..1);
 // fp16/bf16 operands (8-11 mantissa bits) would move that decision, and the reference computes it in fp32.
+#include <algorithm>
 #include <cmath>
+#include <cstdint>
 
 #include "common.h"
 
@@ -150,15 +152,17 @@ __global__ void __launch_bounds__(128) rows_l2_normalize_kernel(float* __restric
 }
 
 // sums[c][:] += sum of the rows x[order[s]] for s in [seg[c], seg[c+1]) in that order (order = points sorted by label):
-// one thread per (cluster, dimension), rows added sequentially -> bit-reproducible, unlike atomics.
+// one thread per (cluster, dimension), rows added sequentially -> bit-reproducible, unlike atomics.  Clusters on grid x (up to
+// 2^31 - 1 of them), 256-wide dimension blocks on grid y, striding when d needs more than 65535 of them.
 __global__ void __launch_bounds__(256) cluster_sum_kernel(const float* __restrict__ x, const long long* __restrict__ order, const long long* __restrict__ seg,
                                                           int d, float* __restrict__ sums) {
-  const int c = blockIdx.y;
-  const int dim = blockIdx.x * 256 + threadIdx.x;
-  if (dim >= d) return;
-  float s = 0.f;
-  for (long long t = seg[c]; t < seg[c + 1]; ++t) s += x[(size_t)order[t] * d + dim];
-  sums[(size_t)c * d + dim] += s;
+  const int c = blockIdx.x;
+  const long long t0 = seg[c], t1 = seg[c + 1];
+  for (long long dim = blockIdx.y * 256ll + threadIdx.x; dim < d; dim += gridDim.y * 256ll) {
+    float s = 0.f;
+    for (long long t = t0; t < t1; ++t) s += x[(size_t)order[t] * d + dim];
+    sums[(size_t)c * d + dim] += s;
+  }
 }
 
 }  // namespace cb
@@ -169,6 +173,7 @@ int cb_rowdot_argmax(cb_ctx* ctx, const float* a, int na, const float* b, int nb
                      int* out_idx, void* stream) {
   if (!ctx) return CB_ERR_ARG;
   if (!a || !b || !out_val || !out_idx) return cb::fail(ctx, CB_ERR_ARG, "rowdot_argmax: null operand");
+  if (((uintptr_t)a | (uintptr_t)b) & 15) return cb::fail(ctx, CB_ERR_ARG, "rowdot_argmax: a and b must be 16-byte aligned (float4 loads)");
   if (nb <= 0) return CB_OK;
   if (na < 0 || d <= 0 || d % 16) return cb::fail(ctx, CB_ERR_UNSUPPORTED, "rowdot_argmax: d=%d must be a positive multiple of 16", d);
   if ((flags & CB_ROWDOT_UPPER) && (a != b || na != nb)) return cb::fail(ctx, CB_ERR_ARG, "rowdot_argmax: CB_ROWDOT_UPPER needs a == b");
@@ -196,7 +201,7 @@ int cb_cluster_sums(cb_ctx* ctx, const float* x, const long long* order, const l
   if (!x || !order || !seg || !sums || n_clusters <= 0 || d <= 0) return cb::fail(ctx, CB_ERR_ARG, "cluster_sums: bad argument");
   CB_CUDA(ctx, cudaSetDevice(ctx->device));
   cb::mark_launch(ctx, CB_PROF_OTHER, (cudaStream_t)stream);
-  cb::cluster_sum_kernel<<<dim3((d + 255) / 256, n_clusters), 256, 0, (cudaStream_t)stream>>>(x, order, seg, d, sums);
+  cb::cluster_sum_kernel<<<dim3(n_clusters, std::min((d - 1) / 256 + 1, 65535)), 256, 0, (cudaStream_t)stream>>>(x, order, seg, d, sums);
   CB_CUDA(ctx, cudaGetLastError());
   return CB_OK;
 }

@@ -352,7 +352,10 @@ int cb_transnet_head(cb_ctx* ctx, const float* h, const float* w, float bias, in
 #define CB_ROWDOT_CLIP 2  /* clamp scores to [-1, 1] before comparing */
 /* For every row j of b[nb][d]: the maximum over rows i of a[na][d] of (a_i . b_j + bias_i) and the FIRST index attaining
  * it; a candidate must be strictly greater than init_val, else out_idx[j] = -1 and out_val[j] = init_val.  All pointers
- * are device fp32 / int32, d a multiple of 16.  Replaces the tiled `E[i0:i1] @ E[j0:j1].T -> clip -> argmax -> where`
+ * are device fp32 / int32, d a multiple of 16 (else CB_ERR_UNSUPPORTED); a and b must be 16-byte aligned, a null or
+ * misaligned operand returns CB_ERR_ARG, nb == 0 is a no-op.  Each score is one fp32 fma chain over d in index order, then
+ * + bias_i.  A candidate row holding a NaN is never returned: its NaN scores fail the `>` test; under CLIP they clamp to -1,
+ * which can only be taken when init_val < -1.  Replaces the tiled `E[i0:i1] @ E[j0:j1].T -> clip -> argmax -> where`
  * loop of SemanticDedupActor.dedup (cosmos_curate/pipelines/video/dedup/dedup_actor.py:420-462) with UPPER|CLIP and
  * init_val = -1, and the nearest-centroid assignment of its KMeansMG call (:232-241) with bias_i = -|c_i|^2 / 2. */
 int cb_rowdot_argmax(cb_ctx* ctx, const float* a, int na, const float* b, int nb, int d, const float* bias, int flags, float init_val, float* out_val,
@@ -360,7 +363,8 @@ int cb_rowdot_argmax(cb_ctx* ctx, const float* a, int na, const float* b, int nb
 /* x[row] /= max(|x[row]|_2, 1e-12) in place (dedup_actor.py:224-225, :407-408); norms_out (nullable) receives |x[row]|. */
 int cb_rows_l2_normalize(cb_ctx* ctx, float* x, int rows, int d, float* norms_out, void* stream);
 /* sums[c][:] += sum of x[order[t]][:] for t in [seg[c], seg[c+1]): the centroid-update reduction of k-means, rows added
- * in the given order by one thread per (cluster, dimension) - bit-reproducible.  order/seg are device int64. */
+ * in the given order to 0.0f by one thread per (cluster, dimension), then added once to sums - bit-reproducible.  order/seg
+ * are device int64.  Any n_clusters >= 1 launches (no grid limit); n_clusters or d <= 0 is CB_ERR_ARG. */
 int cb_cluster_sums(cb_ctx* ctx, const float* x, const long long* order, const long long* seg, int n_clusters, int d, float* sums, void* stream);
 
 /* ---- building blocks exported for the parity tests ------------------------------------------------ */

@@ -82,7 +82,7 @@ def test_kmeans_properties_and_determinism(ctx):  # noqa: F811
     from oracle import dedup as od
 
     rng = np.random.default_rng(8)
-    k, d, n = 12, 80, 5000  # d = 80: exercises the pad-to-16 path
+    k, d, n = 12, 80, 5000  # d = 80 is a multiple of 16: no padding (test_gpu_dedup_exact.py runs the pad-to-16 path at d = 72)
     centers = rng.standard_normal((k, d)).astype(np.float32)
     x = centers[rng.integers(0, k, n)] + 0.3 * rng.standard_normal((n, d)).astype(np.float32)
     r1 = dedup.spherical_kmeans(x, k, max_iter=50, seed=4, ctx=ctx)
